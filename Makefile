@@ -3,13 +3,13 @@ PY ?= python
 
 .PHONY: build test test-gpu bench lint sanitize-host clean
 
-build:            ## sm_100a CUDA extension + C++ host runtime + experimental kernels, in-tree (no GPU needed)
+build:            ## sm_90a CUDA extension + C++ host runtime + experimental kernels, in-tree (no GPU needed)
 	$(PY) -c "import __graft_entry__ as g; g.build()"
 
 test:             ## CPU suite (multi-process gloo tests, emulated sm100 engine, parsers, tools)
 	$(PY) -m pytest tests -x -q -m "not gpu"
 
-test-gpu:         ## on a B200
+test-gpu:         ## on an H100
 	$(PY) -m pytest tests -x -q -m gpu
 
 bench:            ## AlexNet b=256, one GPU -> one JSON line

@@ -48,6 +48,9 @@ def parse_args():
     ap.add_argument("--no-exposed-comm", action="store_true",
                     help="skip the compute-only arm (N > 1) that exposed_comm_ms is measured against")
     ap.add_argument("--require-nvls", action="store_true", help="fail if the arena has no NVLS multicast mapping")
+    ap.add_argument("--dump-outputs", default="", metavar="DIR",
+                    help="after the timed steps, write what the last timed step computed (loss, every learnable blob) "
+                         "as DIR/<name>.npy; blobs over the budget are a fixed seeded sample")
     ap.add_argument("--kernel-list", default="", help="write a per-kernel time table (CUPTI via torch.profiler, a few EAGER "
                     "steps on every rank, rank r -> FILE.r) — works for multi-rank runs, where ncu cannot be used")
     return ap.parse_args()
@@ -108,7 +111,7 @@ class ClockSampler:
 def reference_unavailable():
     why = ("petuum/poseidon cannot be built offline: needs the un-vendored petuum/third_party bundle (zmq, glog, gflags, "
            "leveldb, lmdb, hdf5, opencv, protobuf-dev), cuDNN R2/R3 APIs removed since cuDNN 8, and sm_20..sm_50 "
-           "gencodes rejected by nvcc 12.9; `pip install /root/reference` has no setup.py/pyproject (see DESIGN.md)")
+           "gencodes rejected by nvcc 12.9; the reference tree has no setup.py/pyproject to install it with (see DESIGN.md)")
     print(json.dumps({"impl": "reference", "unavailable": why}))
 
 
@@ -156,6 +159,32 @@ def dump_kernel_list(args, rc, path):
             f.write(f"{e.device_time_total / steps:10.1f} {e.count / steps:10.1f} "
                     f"{e.device_time_total / max(e.count, 1):9.1f}  {e.key[:150]}\n")
     solver.close()
+
+
+DUMP_BUDGET_BYTES = 64 << 20
+
+
+def dump_outputs(solver, out_dir):
+    """What a caller of the timed step gets back from its last step: the loss and the updated learnable blobs (Caffe
+    layout, float32, as a snapshot writes them).  A blob larger than its share of the 64 MB budget is replaced by a
+    sample at fixed indices (seeded by the blob's name, so two builds sample the same elements); the indices are
+    written beside it as <name>.idx.npy."""
+    import re
+    import zlib
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    blobs = [(f"{lname}.{j}", layer, j) for lname, layer in zip(solver.net.layer_names, solver.net.layers)
+             for j in range(len(layer.blobs))]
+    cap = max(1, (DUMP_BUDGET_BYTES - 4096) // 12 // max(1, len(blobs)))     # 4 B value + 8 B index per sampled element
+    np.save(os.path.join(out_dir, "loss.npy"), np.asarray([float(solver.last_loss)], dtype=np.float64))
+    for name, layer, j in blobs:
+        a = np.ascontiguousarray(layer.export_blob(j), dtype=np.float32).reshape(-1)
+        fn = re.sub(r"[^A-Za-z0-9_.-]", "_", name)
+        if a.size > cap:
+            idx = np.sort(np.random.default_rng(zlib.crc32(name.encode())).choice(a.size, cap, replace=False))
+            np.save(os.path.join(out_dir, fn + ".idx.npy"), idx.astype(np.int64))
+            a = a[idx]
+        np.save(os.path.join(out_dir, fn + ".npy"), a)
 
 
 def build_solver(args, rank_ctx, device_resident: bool):
@@ -273,8 +302,8 @@ def main():
     if rc.device.type != "cuda":
         use_graph = False
     if use_graph and args.engine == "torch" and world > 1:
-        # capturing NCCL collectives hung in this image (2 x B200, round 2 call 56: both ranks stuck inside the capture until
-        # the timeout) — the multi-GPU vendor arm runs eager; at 1 GPU graph vs eager differ by 3 % (18.9 vs 19.5 ms AlexNet)
+        # capturing NCCL collectives has hung (both ranks stuck inside the capture until the timeout) — the multi-GPU
+        # vendor arm runs eager
         if rc.is_root:
             print("[bench] vendor arm on >1 GPU: NCCL capture is unreliable here, running eager", file=sys.stderr)
         use_graph = False
@@ -293,6 +322,8 @@ def main():
         sampler.start()
     counting.reset()
     ms, _ = timed_steps(solver, rc, args.steps, read_loss=False)
+    if args.dump_outputs and rc.is_root:
+        dump_outputs(solver, args.dump_outputs)
     launches = counting.total() + (args.steps * getattr(solver, 'graph_launches', 0) if use_graph else 0)
     clocks = sampler.stop() if rc.is_root else None
     value = batch * world * args.steps / (ms / 1e3)
@@ -337,7 +368,7 @@ def main():
                                       ("+sfb" if any(v == "sfb" for v in sfb_layers.values()) and world > 1 else ""),
                        "engine": args.engine, "comm": solver.comm_name, "cuda_graph": bool(use_graph),
                        "solver": "SGD momentum 0.9 wd 5e-4 (reference solver.prototxt)",
-                       "l2": "per-step working set (weights+history+grads+activations) >> 126 MB L2; "
+                       "l2": "per-step working set (weights+history+grads+activations) >> 50 MB L2; "
                              "inputs rotate over 4 batches",
                        "sfb_layers": sfb_layers, "wire_bytes_total": wire,
                        "baseline_ref": "133 img/s per K20 derived in BASELINE.md §1 (reference publishes no img/s)"},

@@ -1,4 +1,4 @@
-"""Standalone conv micro-benchmark (AlexNet shapes) for ncu captures and CUDA-event timings."""
+"""Standalone conv micro-benchmark (AlexNet shapes): CUDA-event timings."""
 import sys
 import torch
 sys.path.insert(0, ".")
@@ -12,7 +12,7 @@ CASES = {
     "conv3": (256, 256, 13, 13, 384, 3, 1, 1, 1),
     "conv4": (256, 384, 13, 13, 384, 3, 1, 1, 2),
     "conv5": (256, 384, 13, 13, 256, 3, 1, 1, 2),
-    # experiments (profiles/r2_conv_ncu_summary.md): same GEMM extent as conv3 (M 43264, N 384, K 2304) with ...
+    # experiments: same GEMM extent as conv3 (M 43264, N 384, K 2304) with ...
     "conv3_nopad": (256, 256, 15, 15, 384, 3, 1, 0, 1),       # ... no padding: no zero-filled pixels in the im2col boxes
     "conv3_as1x1": (256, 2304, 13, 13, 384, 1, 1, 0, 1),      # ... one tap over 2304 channels: im2col-mode TMA reading a plain [M, K] matrix
 }

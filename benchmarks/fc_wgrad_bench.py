@@ -1,6 +1,6 @@
 """Inner-product weight gradient dW[N, K] = dY^T[N, M] · X[M, K] (fp32 output, batch M = 256 rows of reduction):
 output-bound — 151 MB of fp32 for AlexNet fc6 against 19 GFLOP.
-    python benchmarks/fc_wgrad_bench.py [iters]        (under ncu: -k regex:umma_gemm -s 4 -c 1)
+    python benchmarks/fc_wgrad_bench.py [iters]
 """
 import sys
 import torch

@@ -1,4 +1,4 @@
-"""Plain tcgen05 GEMM micro-benchmark: TFLOP/s of the four operand-major combinations and tile widths.
+"""Plain wgmma GEMM micro-benchmark: TFLOP/s of the four operand-major combinations and tile widths.
 
 Separates "how fast is the TMA/MMA/epilogue core" from "how fast is the conv gather" when reading conv numbers.
     python benchmarks/gemm_bench.py [M N K] [iters]

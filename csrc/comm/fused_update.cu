@@ -18,7 +18,7 @@
 #include <torch/library.h>
 #include <torch/types.h>
 
-#include "../gemm/sm100_prims.cuh"
+#include "../gemm/sm90_prims.cuh"
 
 namespace psd {
 
@@ -127,7 +127,7 @@ void fused_update(at::Tensor w, at::Tensor g, at::Tensor h, c10::optional<at::Te
                         reinterpret_cast<uintptr_t>(h.data_ptr())) % 16 == 0 &&
                        (wbp == nullptr || reinterpret_cast<uintptr_t>(wbp) % 8 == 0);
   TORCH_CHECK(aligned, "fused_update: 16-byte aligned buffers expected");
-  const int grid = static_cast<int>(std::max<long>(1, std::min<long>((n / 4 + 255) / 256, 148 * 8)));
+  const int grid = static_cast<int>(std::max<long>(1, std::min<long>((n / 4 + 255) / 256, 132 * 8)));
   const UpdateHyper hp = make_hyper(lr, momentum, decay, rule, l1, delta, gscale);
   const float* lrp = lr_dev.has_value() ? lr_dev->data_ptr<float>() : nullptr;
   auto st = at::cuda::getCurrentCUDAStream();
@@ -137,8 +137,8 @@ void fused_update(at::Tensor w, at::Tensor g, at::Tensor h, c10::optional<at::Te
 }
 
 // ------------------------------------------------------------------------------------ single GPU, many tensors, one launch
-// GoogLeNet steps 128 parameter tensors, most of them a few KB: at ~3 us per launch the optimizer was 7 % of the step
-// (profiles/r2_kernels_googlenet_1gpu.txt).  One launch walks up to kMaxMulti tensors: every block owns a fixed-size
+// GoogLeNet steps 128 parameter tensors, most of them a few KB: one launch per tensor would make launch latency a visible
+// part of the step.  One launch walks up to kMaxMulti tensors: every block owns a fixed-size
 // chunk of one tensor (block -> tensor through a prefix table in the kernel parameters).
 constexpr int kMaxMulti = 48;
 constexpr int kMultiChunk4 = 2048;          // float4 per block-chunk (32 KB of weights)

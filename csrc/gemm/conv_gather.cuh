@@ -1,6 +1,6 @@
 // Implicit-GEMM convolution operand gather (im2col never materialised).
 //
-// Eight producer warps (256 threads) build, directly in the 128B-swizzled shared-memory layout the UMMA
+// Four producer warps (128 threads) build, directly in the 128B-swizzled shared-memory layout the wgmma
 // descriptors expect, 64-element K slices of the virtual im2col matrix
 //        A[m, k],   m = (n, oh, ow),   k = (r, s, c)          (NHWC input, channels innermost)
 // with 16-byte cp.async copies (zero-fill for padding taps / tails).  Two addressing modes:
@@ -8,12 +8,11 @@
 //   ROW : first layers (C padded to 4): the S*C elements of one kernel row are contiguous in memory, so
 //         K is organised as [R][Lp] (Lp = S*C rounded up to 8; the pad multiplies zero weights).
 //
-// Thread mapping (coalescing): thread t owns chunk column j = t & 7 and rows (t >> 3) + 32*i.  A warp-level
+// Thread mapping (coalescing): thread t owns chunk column j = t & 7 and rows (t >> 3) + 16*i.  A warp-level
 // cp.async therefore covers 4 rows x 128 contiguous bytes (4-8 L1 wavefronts) instead of 32 scattered 16-byte
 // pieces (32 wavefronts).
 //
-// The producers are instruction-issue bound (ncu: ~150 SASS instructions per thread per k-block for fprop, ~260
-// for wgrad, vs. a 512-cycle MMA), so everything that depends only on the row m is taken out of the loop: a
+// The producers are instruction-issue bound, so everything that depends only on the row m is taken out of the loop: a
 // per-geometry ROW TABLE (8 bytes per output pixel, built once by conv_rowtab_kernel and cached on the host side)
 // holds the element offset of tap (0,0) and a validity bit mask per kernel row / kernel column.  Per chunk the
 // producer then needs one AND/compare for the bounds check and one add for the address.
@@ -25,7 +24,7 @@
 // (reference: src/caffe/util/im2col.cu:12-132, src/caffe/layers/conv_layer.cu:13-119).
 #pragma once
 #include "fastdiv.cuh"
-#include "sm100_prims.cuh"
+#include "sm90_prims.cuh"
 
 namespace psd {
 

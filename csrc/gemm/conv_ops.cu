@@ -1,4 +1,4 @@
-// Implicit-GEMM convolution on the tcgen05 GEMM core: fprop, dgrad (stride 1), wgrad (split-K fp32 atomics).
+// Implicit-GEMM convolution on the wgmma GEMM core: fprop, dgrad (stride 1), wgrad (split-K, partials summed in order).
 //
 // Layouts (sm100 engine): activations NHWC bf16 (pixel pitch may exceed C for channel-slice views);
 // weights fp32 master + bf16 shadow as [Cout][R][S][Cg] ("KRSC", K-major rows of length R*S*Cg), or
@@ -16,7 +16,7 @@
 #include <mutex>
 
 #include "../ops/nhwc_common.cuh"
-#include "umma_gemm.cuh"
+#include "wgmma_gemm.cuh"
 
 namespace psd {
 
@@ -26,10 +26,11 @@ void encode_tmap_bf16_3d(CUtensorMap* map, const void* base, int64_t d0, int64_t
                          int box0, int box1, int box2);
 void encode_tmap_im2col_bf16(CUtensorMap* map, const void* base, int64_t C, int64_t W, int64_t H, int64_t N, int64_t pitch,
                              int lower_w, int lower_h, int upper_w, int upper_h, int pixels, int stride_w, int stride_h);
+void splitk_reduce(const at::Tensor& ws, int splits, float* out, long ldo, int M, int N, cudaStream_t stream);
 
 static int g_conv_im2col = 1;      // TMA im2col-mode operand fetch where the geometry allows it (C_g % 64 == 0)
 
-static int g_conv_cluster = 1;     // CTAs per cluster sharing the TMA operand by multicast (1 = off; measured slower at 2 on B200, kept as an option)
+static int g_conv_cluster = 1;     // CTAs per cluster sharing the TMA operand by multicast (1 = off)
 
 int pair_cta_enabled();
 extern int g_max_stages;
@@ -37,7 +38,7 @@ extern int g_no_bulk_epi;
 
 template <int BN, bool A_MN, bool B_MN, int EPI, int GATHER, int CG = 1>
 static void launch_conv(const TmapSet& tm, const GemmParams& p, const ConvGeom& cg, int grid, cudaStream_t stream) {
-  auto kern = umma_gemm_kernel<BN, A_MN, B_MN, EPI, GATHER, CG>;
+  auto kern = wgmma_gemm_kernel<BN, A_MN, B_MN, EPI, GATHER, CG>;
   constexpr int smem = GemmSmem<BN, CG>::kTotal;
   static bool configured = false;
   if (!configured) {
@@ -49,6 +50,14 @@ static void launch_conv(const TmapSet& tm, const GemmParams& p, const ConvGeom& 
   if (cluster <= 1) {
     kern<<<grid, threads, smem, stream>>>(tm, p, cg);
   } else {
+    static std::map<int, int> resident;                 // per cluster size (conv clusters come in 2, 3 and 4)
+    static std::mutex mu;
+    {
+      std::lock_guard<std::mutex> lock(mu);
+      auto it = resident.find(cluster);
+      if (it == resident.end()) it = resident.emplace(cluster, resident_cluster_ctas(kern, threads, smem, cluster)).first;
+      grid = std::min(grid, it->second);
+    }
     cudaLaunchConfig_t cfg{};
     cfg.gridDim = dim3(grid);
     cfg.blockDim = dim3(threads);
@@ -66,29 +75,28 @@ static void launch_conv(const TmapSet& tm, const GemmParams& p, const ConvGeom& 
   C10_CUDA_KERNEL_LAUNCH_CHECK();
 }
 
-// Grid of a paired-CTA launch: one CTA pair per pair-tile, at most sms/2 pairs.
+// Grid of a CTA-pair launch: one CTA pair per pair-tile, at most sms/2 pairs.
 static int pair_grid(long m_blocks, long n_blocks, long split, int sms) {
   const long pair_tiles = ((m_blocks + 1) / 2) * n_blocks * split;
   return static_cast<int>(2 * std::max<long>(1, std::min<long>(pair_tiles, sms / 2)));
 }
 
 static int g_conv_mcast = 1;       // CTAs per cluster sharing the im2col operand by TMA multicast (1 = off, the default:
-                                   // measured no faster on B200 — every SM still ingests the whole tile, profiles/r2_conv_ncu_summary.md)
-static int g_conv_pair = 1;        // paired CTAs for the im2col convolution kernels: A/B on one box (r2 call 13) AlexNet
-                                   // 3.298 -> 3.267 ms, VGG-16 10.49 -> 10.04 ms per step
+                                   // every SM still ingests the whole tile)
+static int g_conv_pair = 1;        // CTA pairs sharing the weight / im2col B tile for the im2col convolution kernels
 
-// Launch the im2col-A kernel (fprop / dgrad) for tile width bn; CG = 2: paired CTAs, else cluster multicast (p.cluster).
+// Launch the im2col-A kernel (fprop / dgrad) for tile width bn; CG = 2: CTA pairs, else cluster multicast (p.cluster).
 template <int CG>
 static void launch_im2col_a(int bn, const TmapSet& tm, const GemmParams& p, const ConvGeom& cg, int grid, cudaStream_t stream) {
   switch (bn) {
     case 32:
       if constexpr (CG == 1) launch_conv<32, false, false, EPI_BF16, IM2COL_A, 1>(tm, p, cg, grid, stream);
-      else TORCH_CHECK(false, "paired CTAs: BLOCK_N >= 64");
+      else TORCH_CHECK(false, "CTA pairs: BLOCK_N >= 64");
       break;
     case 64: launch_conv<64, false, false, EPI_BF16, IM2COL_A, CG>(tm, p, cg, grid, stream); break;
     case 96:
       if constexpr (CG == 1) launch_conv<96, false, false, EPI_BF16, IM2COL_A, 1>(tm, p, cg, grid, stream);
-      else TORCH_CHECK(false, "paired CTAs: BLOCK_N 96 is not instantiated");
+      else TORCH_CHECK(false, "CTA pairs: BLOCK_N 96 is not instantiated");
       break;
     case 128: launch_conv<128, false, false, EPI_BF16, IM2COL_A, CG>(tm, p, cg, grid, stream); break;
     case 192: launch_conv<192, false, false, EPI_BF16, IM2COL_A, CG>(tm, p, cg, grid, stream); break;
@@ -99,8 +107,7 @@ static void launch_im2col_a(int bn, const TmapSet& tm, const GemmParams& p, cons
 
 // Multicast plan for an im2col-A convolution with n_cols output columns: the cluster's C CTAs take C consecutive column
 // blocks of the SAME pixel tile and each fetches 128 / C of its pixel rows.  The tile width is the narrowest
-// instantiated one that covers n_cols / C (the TMA time per k-block is ~815 / C cycles, the MMA time 2 * bn: narrow
-// tiles cost nothing while the TMA engine is the bound).  Returns C (1 = no multicast) and sets *bn, *grid.
+// instantiated one that covers n_cols / C.  Returns C (1 = no multicast) and sets *bn, *grid.
 static int plan_im2col_mcast(long n_cols, long m_blocks, int sms, int* bn, int* grid) {
   int c = g_conv_mcast;
   if (c <= 1 || n_cols < 32) return 1;
@@ -113,7 +120,7 @@ static int plan_im2col_mcast(long n_cols, long m_blocks, int sms, int* bn, int* 
   *bn = w;
   const long n_blocks = (n_cols + w - 1) / w;
   const long cluster_tiles = m_blocks * ((n_blocks + c - 1) / c);
-  const int usable = c >= 4 ? ((sms / 4) * 4 - 16) : (sms / c) * c;       // size-4 clusters strand ~16 SMs (GPC shapes)
+  const int usable = (sms / c) * c;             // launch_conv caps the grid at the clusters that fit at once
   *grid = static_cast<int>(std::max<long>(c, std::min<long>(cluster_tiles * c, (usable / c) * c)));
   return c;
 }
@@ -122,7 +129,7 @@ static int plan_im2col_mcast(long n_cols, long m_blocks, int sms, int* bn, int* 
 static int pick_cluster(long tiles_along, long tiles_total, int sms, int* grid) {
   int c = g_conv_cluster;
   while (c > 1 && tiles_along < c) c >>= 1;
-  const int usable = c >= 4 ? (sms / 4) * 4 - 16 : sms;      // size-4 clusters strand ~16 SMs (GPC shapes)
+  const int usable = sms;                       // launch_conv caps the grid at the clusters that fit at once
   const long ctiles = (tiles_total + c - 1) / c;              // cluster tiles (upper bound incl. edge padding)
   long g = std::min<long>(ctiles * c, (usable / c) * c);
   g = std::max<long>(c, (g / c) * c);
@@ -199,14 +206,19 @@ static ConvGeom make_geom(const at::Tensor& x, const NhwcView& xv, int c_off, in
 
 // TMA im2col eligibility: TAP mode, 64-channel K slices never straddle a tap, corner offsets fit the descriptor.
 // On success fills `map` for boxes of `pixels` base pixels x 64 channels over the gathered tensor.
-static bool try_im2col_map(CUtensorMap* map, const ConvGeom& g, int pixels) {
+static bool im2col_ok(const ConvGeom& g) {
   if (!g_conv_im2col || g.mode != 0 || g.Cgk % 64 != 0) return false;
   const int org_w = g.off_w - (g.dr < 0 ? g.S - 1 : 0), org_h = g.off_h - (g.dr < 0 ? g.R - 1 : 0);
   // the bounding box must enumerate exactly OW x OH base pixels: extent + upper - lower - 1 = (O - 1) * stride
   const int up_w = (g.OW - 1) * g.sw + 1 + org_w - g.W, up_h = (g.OH - 1) * g.sh + 1 + org_h - g.H;
   auto ok = [](int v) { return v >= -128 && v <= 127; };
   if (!ok(org_w) || !ok(org_h) || !ok(up_w) || !ok(up_h) || g.sw > 8 || g.sh > 8) return false;
-  if ((reinterpret_cast<uintptr_t>(g.x) & 15) != 0 || (g.pitch * 2) % 16 != 0) return false;
+  return (reinterpret_cast<uintptr_t>(g.x) & 15) == 0 && (g.pitch * 2) % 16 == 0;
+}
+static bool try_im2col_map(CUtensorMap* map, const ConvGeom& g, int pixels) {
+  if (!im2col_ok(g)) return false;
+  const int org_w = g.off_w - (g.dr < 0 ? g.S - 1 : 0), org_h = g.off_h - (g.dr < 0 ? g.R - 1 : 0);
+  const int up_w = (g.OW - 1) * g.sw + 1 + org_w - g.W, up_h = (g.OH - 1) * g.sh + 1 + org_h - g.H;
   encode_tmap_im2col_bf16(map, g.x, g.Cg, g.W, g.H, g.N, g.pitch, org_w, org_h, up_w, up_h, pixels, g.sw, g.sh);
   return true;
 }
@@ -250,7 +262,8 @@ at::Tensor conv_fprop(const at::Tensor& x, const at::Tensor& wb, const c10::opti
     ConvGeom cg = make_geom(x, xv, gidx * Cg, Cg, OH, OW, d, false, Cgk);
     TORCH_CHECK(wb.size(1) == cg.K, "conv_fprop: weight K ", wb.size(1), " != expected ", cg.K);
     const long m_blocks = (cg.M + BLOCK_M - 1) / BLOCK_M;
-    const int bn = pick_conv_bn(Cout_g, m_blocks, sms);
+    int bn = pick_conv_bn(Cout_g, m_blocks, sms);
+    if (!(g_conv_cluster == 1 && im2col_ok(cg))) bn = std::min(bn, kGatherMaxBN);
     const long n_blocks = (Cout_g + bn - 1) / bn;
     int grid = 0;
     const int cl = pick_cluster(m_blocks, m_blocks * n_blocks, sms, &grid);
@@ -285,7 +298,7 @@ at::Tensor conv_fprop(const at::Tensor& x, const at::Tensor& wb, const c10::opti
         continue;
       }
       if (g_conv_pair && pair_cta_enabled() && m_blocks >= 2 && bn >= 64) {
-        // paired CTAs: two pixel blocks share every weight tile; each CTA stages BN/2 weight rows
+        // CTA pairs: two pixel blocks share every weight tile; each CTA fetches BN/2 weight rows for both
         encode_tmap_bf16_2d(&tm.b[0], wptr, cg.K, Cout_g, cg.K, BLOCK_K, bn / 2);
         launch_im2col_a<2>(bn, tm, p, cg, pair_grid(m_blocks, n_blocks, 1, sms), stream);
         continue;
@@ -294,12 +307,8 @@ at::Tensor conv_fprop(const at::Tensor& x, const at::Tensor& wb, const c10::opti
       continue;
     }
     TORCH_CHECK(cg.Cgk == cg.Cg, "conv_fprop: channel-padded operand needs the TMA im2col path");
-    switch (bn) {
-      case 64: launch_conv<64, false, false, EPI_BF16, GATHER_A>(tm, p, cg, grid, stream); break;
-      case 128: launch_conv<128, false, false, EPI_BF16, GATHER_A>(tm, p, cg, grid, stream); break;
-      case 192: launch_conv<192, false, false, EPI_BF16, GATHER_A>(tm, p, cg, grid, stream); break;
-      default: launch_conv<256, false, false, EPI_BF16, GATHER_A>(tm, p, cg, grid, stream); break;
-    }
+    if (bn == 64) launch_conv<64, false, false, EPI_BF16, GATHER_A>(tm, p, cg, grid, stream);
+    else launch_conv<128, false, false, EPI_BF16, GATHER_A>(tm, p, cg, grid, stream);
   }
   return y;
 }
@@ -330,7 +339,8 @@ at::Tensor conv_dgrad(const at::Tensor& dy, const at::Tensor& wt, at::IntArrayRe
     ConvGeom cg = make_geom(dy, dv, gidx * Cout_g, Cout_g, H, W, d, true, Cok);
     TORCH_CHECK(wt.size(1) == cg.K, "conv_dgrad: packed weight K mismatch");
     const long m_blocks = (cg.M + BLOCK_M - 1) / BLOCK_M;
-    const int bn = pick_conv_bn(Cg, m_blocks, sms);
+    int bn = pick_conv_bn(Cg, m_blocks, sms);
+    if (!(g_conv_cluster == 1 && im2col_ok(cg))) bn = std::min(bn, kGatherMaxBN);
     const long n_blocks = (Cg + bn - 1) / bn;
     int grid = 0;
     const int cl = pick_cluster(m_blocks, m_blocks * n_blocks, sms, &grid);
@@ -372,12 +382,8 @@ at::Tensor conv_dgrad(const at::Tensor& dy, const at::Tensor& wt, at::IntArrayRe
       continue;
     }
     TORCH_CHECK(cg.Cgk == cg.Cg, "conv_dgrad: channel-padded operand needs the TMA im2col path");
-    switch (bn) {
-      case 64: launch_conv<64, false, false, EPI_BF16, GATHER_A>(tm, p, cg, grid, stream); break;
-      case 128: launch_conv<128, false, false, EPI_BF16, GATHER_A>(tm, p, cg, grid, stream); break;
-      case 192: launch_conv<192, false, false, EPI_BF16, GATHER_A>(tm, p, cg, grid, stream); break;
-      default: launch_conv<256, false, false, EPI_BF16, GATHER_A>(tm, p, cg, grid, stream); break;
-    }
+    if (bn == 64) launch_conv<64, false, false, EPI_BF16, GATHER_A>(tm, p, cg, grid, stream);
+    else launch_conv<128, false, false, EPI_BF16, GATHER_A>(tm, p, cg, grid, stream);
   }
   return dx;
 }
@@ -404,7 +410,7 @@ bool conv_dgrad_w_impl(const at::Tensor& dy, const at::Tensor& wb, at::IntArrayR
     if (!try_im2col_map(&tm.a[0], cg, BLOCK_M)) return false;
     const long m_blocks = (cg.M + BLOCK_M - 1) / BLOCK_M;
     int bn = pick_conv_bn(Cg, m_blocks, sms);
-    if (bn == 192) bn = 256;                       // MN-major B: whole 64-column chunks per CTA (and per pair half)
+    if (bn == 192) bn = 256;                       // MN-major B: whole 64-column chunks per CTA pair half
     const long n_blocks = (Cg + bn - 1) / bn;
     const __nv_bfloat16* wptr = reinterpret_cast<const __nv_bfloat16*>(wb.data_ptr()) + static_cast<long>(gidx) * Cout_g * RS * Cg;
     encode_tmap_bf16_3d(&tm.b[0], wptr, Cg, Cout_g, RS, static_cast<int64_t>(RS) * Cg, Cg, 64, 64, 1);
@@ -455,8 +461,8 @@ at::Tensor conv_dgrad_w(const at::Tensor& dy, const at::Tensor& wb, at::IntArray
   return dx;
 }
 
-// dw[Cout, Kw] fp32 += alpha * dYᵀ · im2col(x)   (atomic split-K over the N*OH*OW reduction; dw pre-zeroed
-// unless accumulating into an existing gradient).
+// dw[Cout, Kw] fp32 += alpha * dYᵀ · im2col(x)   (split-K over the N*OH*OW reduction, partials summed in a fixed order;
+// dw pre-zeroed unless accumulating into an existing gradient).
 void conv_wgrad(const at::Tensor& x, const at::Tensor& dy, at::Tensor dw, at::IntArrayRef kernel, at::IntArrayRef stride,
                 at::IntArrayRef pad, int64_t groups, int64_t mode, double alpha, int64_t cgk) {
   TORCH_CHECK(x.is_cuda() && x.scalar_type() == at::kBFloat16 && dy.scalar_type() == at::kBFloat16);
@@ -477,6 +483,7 @@ void conv_wgrad(const at::Tensor& x, const at::Tensor& dy, at::Tensor dw, at::In
     TORCH_CHECK(dw.size(0) == Cout && dw.size(1) == k_real, "conv_wgrad: dw shape mismatch");
     int bn = cg.K > 128 ? 256 : (cg.K > 64 ? 128 : 64);
     if (bn == 256 && ((cg.K + 191) / 192 * 192) * 100 < ((cg.K + 255) / 256 * 256) * 85) bn = 192;   // e.g. K = 576
+    if (!(g_conv_cluster == 1 && im2col_ok(cg))) bn = std::min(bn, kGatherMaxBN);
     TmapSet tm;
     // A = dYᵀ: MN-major, inner = Cout_g channels of this group, outer = M pixels, pitch = dy pixel pitch
     const __nv_bfloat16* dyp = reinterpret_cast<const __nv_bfloat16*>(dy.data_ptr()) + gidx * Cout_g;
@@ -502,44 +509,54 @@ void conv_wgrad(const at::Tensor& x, const at::Tensor& dy, at::Tensor dw, at::In
     if (cg.Cgk != cg.Cg) { p.col_cg = cg.Cg; p.col_cgk = cg.Cgk; }
     p.atomic = 1;
     p.alpha = static_cast<float>(alpha);
-    if (cl == 1 && try_im2col_map(&tm.b[0], cg, BLOCK_K)) {
-      const long m_blocks = (Cout_g + BLOCK_M - 1) / BLOCK_M;
-      if (g_conv_mcast > 1 && m_blocks >= 2 && bn >= 128) {
-        // cluster along Cout: its CTAs need the same im2col B tile (bn / 64 boxes of 64 pixels x 64 channels per k-block,
-        // ~6 cycles per pixel row on the TMA engine) — each fetches every C-th box and multicasts it
-        const int mc = (m_blocks % 3 == 0 && bn >= 192) ? 3 : 2;
-        const long ctiles = ((m_blocks + mc - 1) / mc) * n_blocks * split;
-        p.cluster = mc;
-        const int mgrid = static_cast<int>(std::max<long>(1, std::min<long>(ctiles, sms / mc))) * mc;
-        switch (bn) {
-          case 128: launch_conv<128, true, true, EPI_F32, IM2COL_B>(tm, p, cg, mgrid, stream); break;
-          case 192: launch_conv<192, true, true, EPI_F32, IM2COL_B>(tm, p, cg, mgrid, stream); break;
-          default: launch_conv<256, true, true, EPI_F32, IM2COL_B>(tm, p, cg, mgrid, stream); break;
+    // Split reduction: each split stores its partial to its own workspace slice (plain stores) and the slices are added
+    // onto dw in split order afterwards, so the gradient does not depend on which CTA finishes first.  One split adds
+    // onto dw directly (one add per element).
+    float* const dwg = p.c_f32;
+    at::Tensor ws;
+    if (split > 1) {
+      ws = at::empty({split, Cout_g, k_real}, dw.options());
+      p.c_f32 = ws.data_ptr<float>();
+      p.split_stride = static_cast<long>(Cout_g) * k_real;
+      p.atomic = 0;
+    }
+    [&] {
+      if (cl == 1 && try_im2col_map(&tm.b[0], cg, BLOCK_K)) {
+        const long m_blocks = (Cout_g + BLOCK_M - 1) / BLOCK_M;
+        if (g_conv_mcast > 1 && m_blocks >= 2 && bn >= 128) {
+          // cluster along Cout: its CTAs need the same im2col B tile (bn / 64 boxes of 64 pixels x 64 channels per k-block)
+          // — each fetches every C-th box and multicasts it
+          const int mc = (m_blocks % 3 == 0 && bn >= 192) ? 3 : 2;
+          const long ctiles = ((m_blocks + mc - 1) / mc) * n_blocks * split;
+          p.cluster = mc;
+          const int mgrid = static_cast<int>(std::max<long>(1, std::min<long>(ctiles, sms / mc))) * mc;
+          switch (bn) {
+            case 128: launch_conv<128, true, true, EPI_F32, IM2COL_B>(tm, p, cg, mgrid, stream); break;
+            case 192: launch_conv<192, true, true, EPI_F32, IM2COL_B>(tm, p, cg, mgrid, stream); break;
+            default: launch_conv<256, true, true, EPI_F32, IM2COL_B>(tm, p, cg, mgrid, stream); break;
+          }
+          return;
         }
-        continue;
+        if (g_conv_pair && pair_cta_enabled() && m_blocks >= 2 && m_blocks % 2 == 0 && (bn == 128 || bn == 256)) {
+          // CTA pairs along Cout (even block counts only: a phantom block would waste a third of conv3's MMA work)
+          const int pgrid = pair_grid(m_blocks, n_blocks, split, sms);
+          if (bn == 128) launch_conv<128, true, true, EPI_F32, IM2COL_B, 2>(tm, p, cg, pgrid, stream);
+          else launch_conv<256, true, true, EPI_F32, IM2COL_B, 2>(tm, p, cg, pgrid, stream);
+          return;
+        }
+        switch (bn) {
+          case 64: launch_conv<64, true, true, EPI_F32, IM2COL_B>(tm, p, cg, grid, stream); break;
+          case 128: launch_conv<128, true, true, EPI_F32, IM2COL_B>(tm, p, cg, grid, stream); break;
+          case 192: launch_conv<192, true, true, EPI_F32, IM2COL_B>(tm, p, cg, grid, stream); break;
+          default: launch_conv<256, true, true, EPI_F32, IM2COL_B>(tm, p, cg, grid, stream); break;
+        }
+        return;
       }
-      if (g_conv_pair && pair_cta_enabled() && m_blocks >= 2 && m_blocks % 2 == 0 && (bn == 128 || bn == 256)) {
-        // paired CTAs along Cout (even block counts only: a phantom block would waste a third of conv3's MMA work)
-        const int pgrid = pair_grid(m_blocks, n_blocks, split, sms);
-        if (bn == 128) launch_conv<128, true, true, EPI_F32, IM2COL_B, 2>(tm, p, cg, pgrid, stream);
-        else launch_conv<256, true, true, EPI_F32, IM2COL_B, 2>(tm, p, cg, pgrid, stream);
-        continue;
-      }
-      switch (bn) {
-        case 64: launch_conv<64, true, true, EPI_F32, IM2COL_B>(tm, p, cg, grid, stream); break;
-        case 128: launch_conv<128, true, true, EPI_F32, IM2COL_B>(tm, p, cg, grid, stream); break;
-        case 192: launch_conv<192, true, true, EPI_F32, IM2COL_B>(tm, p, cg, grid, stream); break;
-        default: launch_conv<256, true, true, EPI_F32, IM2COL_B>(tm, p, cg, grid, stream); break;
-      }
-      continue;
-    }
-    TORCH_CHECK(cg.Cgk == cg.Cg, "conv_wgrad: channel-padded reduction needs the TMA im2col path");
-    switch (bn) {
-      case 64: launch_conv<64, true, true, EPI_F32, GATHER_B>(tm, p, cg, grid, stream); break;
-      case 128: launch_conv<128, true, true, EPI_F32, GATHER_B>(tm, p, cg, grid, stream); break;
-      case 192: launch_conv<192, true, true, EPI_F32, GATHER_B>(tm, p, cg, grid, stream); break;
-      default: launch_conv<256, true, true, EPI_F32, GATHER_B>(tm, p, cg, grid, stream); break;
-    }
+      TORCH_CHECK(cg.Cgk == cg.Cg, "conv_wgrad: channel-padded reduction needs the TMA im2col path");
+      if (bn == 64) launch_conv<64, true, true, EPI_F32, GATHER_B>(tm, p, cg, grid, stream);
+      else launch_conv<128, true, true, EPI_F32, GATHER_B>(tm, p, cg, grid, stream);
+    }();
+    if (split > 1) splitk_reduce(ws, static_cast<int>(split), dwg, k_real, Cout_g, static_cast<int>(k_real), stream);
   }
 }
 

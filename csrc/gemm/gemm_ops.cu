@@ -1,14 +1,10 @@
-// Host side of the tcgen05 GEMM family: tensor-map encoding, template dispatch, torch op registration.
+// Host side of the wgmma GEMM family: tensor-map encoding, template dispatch, torch op registration.
 #include <ATen/cuda/CUDAContext.h>
 #include <c10/cuda/CUDAGuard.h>
 #include <torch/library.h>
 #include <torch/types.h>
 
-#include <array>
-#include <map>
-#include <mutex>
-
-#include "umma_gemm.cuh"
+#include "wgmma_gemm.cuh"
 
 namespace psd {
 
@@ -92,18 +88,19 @@ void encode_tmap_im2col_bf16(CUtensorMap* map, const void* base, int64_t C, int6
               " N=", N, " lower=", lower_w, ",", lower_h, " upper=", upper_w, ",", upper_h);
 }
 
-int g_no_bulk_epi = 2;             // bit 0 / 1: fp32 / bf16 outputs NOT through the bulk-store epilogue (bf16: measured slower, off)
+int g_no_bulk_epi = 2;             // bit 0 / 1: fp32 / bf16 outputs NOT through the bulk-store epilogue (bf16: off by default)
 int g_max_stages = 0;             // experiment knob (set_max_stages): ring stages actually used, 0 = all
-static int g_pair_cta = 1;        // cta_group::2 (paired CTAs) where the tile space allows it; 0 = single-CTA kernels only
+static int g_pair_cta = 1;        // CTA pairs sharing the B tile by multicast where the tile space allows it; 0 = single CTAs
 int pair_cta_enabled() { return g_pair_cta; }
 
 // Launch on a (CG,1,1) cluster.  grid is a multiple of CG.
 template <typename Kern>
-static void launch_clustered(Kern kern, int grid, int threads, int smem, int cluster, cudaStream_t stream, const TmapSet& tm,
-                             const GemmParams& p, const ConvGeom& cg) {
+static void launch_clustered(Kern kern, int grid, int threads, int smem, int cluster, int resident, cudaStream_t stream,
+                             const TmapSet& tm, const GemmParams& p, const ConvGeom& cg) {
   if (cluster <= 1) {
     kern<<<grid, threads, smem, stream>>>(tm, p, cg);
   } else {
+    grid = std::min(grid, resident);
     cudaLaunchConfig_t cfg{};
     cfg.gridDim = dim3(grid);
     cfg.blockDim = dim3(threads);
@@ -123,14 +120,16 @@ static void launch_clustered(Kern kern, int grid, int threads, int smem, int clu
 
 template <int BN, bool A_MN, bool B_MN, int EPI, int CG>
 static void launch(const TmapSet& tm, const GemmParams& p, int grid, cudaStream_t stream) {
-  auto kern = umma_gemm_kernel<BN, A_MN, B_MN, EPI, GATHER_NONE, CG>;
+  auto kern = wgmma_gemm_kernel<BN, A_MN, B_MN, EPI, GATHER_NONE, CG>;
   constexpr int smem = GemmSmem<BN, CG>::kTotal;
   static bool configured = false;
+  static int resident = 0;
   if (!configured) {
     C10_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    if (CG > 1) resident = resident_cluster_ctas(kern, kNumThreads, smem, CG);
     configured = true;
   }
-  launch_clustered(kern, grid, kNumThreads, smem, CG, stream, tm, p, ConvGeom{});
+  launch_clustered(kern, grid, kNumThreads, smem, CG, resident, stream, tm, p, ConvGeom{});
 }
 
 template <bool A_MN, bool B_MN, int EPI>
@@ -179,7 +178,7 @@ void gemm_launch(const std::vector<int64_t>& a_ptrs, bool a_mn, int64_t lda, con
   const int sms = prop->multiProcessorCount;
   if (bn <= 0) bn = pick_bn(M, N, sms);
   const int64_t m_blocks = (M + BLOCK_M - 1) / BLOCK_M;
-  // Paired CTAs (cta_group::2): two m-blocks share every B tile.  Needs >= 2 m-blocks, an even CTA budget, and — for an
+  // CTA pairs: two m-blocks share every B tile.  Needs >= 2 m-blocks, an even CTA budget, and — for an
   // MN-major B — a half tile made of whole 64-column chunks.
   int cgp = (g_pair_cta && m_blocks >= 2 && (!b_mn || bn >= 128) && (max_ctas <= 0 || max_ctas >= 2)) ? 2 : 1;
   TmapSet tm;
@@ -218,19 +217,22 @@ void gemm_launch(const std::vector<int64_t>& a_ptrs, bool a_mn, int64_t lda, con
   }
 }
 
-// Split-K finish: out = act(ws + bias) (optionally ReLU-masked) -> bf16, and the fp32 partial-sum workspace is left ZEROED
-// for its next user (the workspace is cached: no memset launch per call).  Four columns per thread (16-byte loads /
-// stores, 32-bit index math); the scalar form serves N or ldc that are not multiples of 4.
+// Split-K finish: out = act(sum_s ws[s] + bias) (optionally ReLU-masked) -> bf16.  ws holds one dense [M, N] fp32 partial per
+// split, summed in split order: the result does not depend on which CTA finished first.  Four columns per thread (16-byte
+// loads / stores, 32-bit index math); the scalar form serves N or ldc that are not multiples of 4.
 __global__ void __launch_bounds__(256)
-splitk_finish_kernel(float* __restrict__ ws, __nv_bfloat16* __restrict__ out, long ldc, const float* __restrict__ bias,
-                     const __nv_bfloat16* __restrict__ mask, int relu, float slope, int M, int N) {
+splitk_finish_kernel(const float* __restrict__ ws, long split_stride, int splits, __nv_bfloat16* __restrict__ out, long ldc,
+                     const float* __restrict__ bias, const __nv_bfloat16* __restrict__ mask, int relu, float slope, int M, int N) {
   if ((N & 3) == 0 && (ldc & 3) == 0) {
     const uint32_t n4 = static_cast<uint32_t>(N) >> 2;
     const uint32_t total4 = static_cast<uint32_t>(M) * n4;
     for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < total4; i += gridDim.x * blockDim.x) {
       const uint32_t m = i / n4, c = (i - m * n4) << 2;
-      float4 v = reinterpret_cast<float4*>(ws)[i];
-      reinterpret_cast<float4*>(ws)[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+      float4 v = reinterpret_cast<const float4*>(ws)[i];
+      for (int sp = 1; sp < splits; ++sp) {
+        const float4 w = reinterpret_cast<const float4*>(ws + sp * split_stride)[i];
+        v.x += w.x; v.y += w.y; v.z += w.z; v.w += w.w;
+      }
       if (bias != nullptr) {
         const float4 b = *reinterpret_cast<const float4*>(bias + c);
         v.x += b.x; v.y += b.y; v.z += b.z; v.w += b.w;
@@ -260,12 +262,33 @@ splitk_finish_kernel(float* __restrict__ ws, __nv_bfloat16* __restrict__ out, lo
        i += static_cast<long>(gridDim.x) * blockDim.x) {
     const int m = static_cast<int>(i / N), n = static_cast<int>(i - static_cast<long>(m) * N);
     float v = ws[i];
-    ws[i] = 0.f;
+    for (int sp = 1; sp < splits; ++sp) v += ws[sp * split_stride + i];
     if (bias != nullptr) v += bias[n];
     if (relu) v = v > 0.f ? v : v * slope;
     if (mask != nullptr && !(__bfloat162float(mask[m * ldc + n]) > 0.f)) v *= slope;
     out[m * ldc + n] = __float2bfloat16(v);
   }
+}
+
+// out[m, n] += sum_s ws[s][m, n] in split order (ws: `splits` dense [M, N] fp32 partials, split_stride elements apart).
+__global__ void __launch_bounds__(256)
+splitk_reduce_kernel(const float* __restrict__ ws, long split_stride, int splits, float* __restrict__ out, long ldo, int M, int N) {
+  const long total = static_cast<long>(M) * N;
+  for (long i = blockIdx.x * static_cast<long>(blockDim.x) + threadIdx.x; i < total;
+       i += static_cast<long>(gridDim.x) * blockDim.x) {
+    const long m = i / N, n = i - m * N;
+    float v = ws[i];
+    for (int sp = 1; sp < splits; ++sp) v += ws[sp * split_stride + i];
+    out[m * ldo + n] += v;
+  }
+}
+
+void splitk_reduce(const at::Tensor& ws, int splits, float* out, long ldo, int M, int N, cudaStream_t stream) {
+  const long total = static_cast<long>(M) * N;
+  const int sms = at::cuda::getCurrentDeviceProperties()->multiProcessorCount;
+  const int grid = static_cast<int>(std::max<long>(1, std::min<long>((total + 255) / 256, sms * 8L)));
+  splitk_reduce_kernel<<<grid, 256, 0, stream>>>(ws.data_ptr<float>(), total, splits, out, ldo, M, N);
+  C10_CUDA_KERNEL_LAUNCH_CHECK();
 }
 
 // ------------------------------------------------------------------------------------ torch ops
@@ -295,9 +318,9 @@ at::Tensor gemm_bf16(const at::Tensor& a, bool a_mn, const at::Tensor& b, bool b
   p.alpha = 1.f;
   p.split_k = 1;
   auto stream = at::cuda::getCurrentCUDAStream();
-  // Small-M GEMMs (the inner-product forward / data-gradient at batch 256): two M blocks cannot fill 148 SMs with wide
-  // tiles, and narrow tiles re-read the activation panel once per 64 output columns (fc6 forward: 53 us against 24 us
-  // for a split-K schedule).  Split the reduction over the idle SMs into an fp32 workspace, then one finishing pass.
+  // Small-M GEMMs (the inner-product forward / data-gradient at batch 256): two M blocks cannot fill the SMs with wide
+  // tiles, and narrow tiles re-read the activation panel once per 64 output columns.  Split the reduction over the idle
+  // SMs into an fp32 workspace, then one finishing pass.
   if (bn <= 0 && !a_mn) {
     const int sms = at::cuda::getCurrentDeviceProperties()->multiProcessorCount;
     const int bn_s = N >= 256 ? 256 : (N > 64 ? 128 : 64);
@@ -305,29 +328,21 @@ at::Tensor gemm_bf16(const at::Tensor& a, bool a_mn, const at::Tensor& b, bool b
     const int64_t kb = (K + BLOCK_K - 1) / BLOCK_K;
     const int64_t split = std::min<int64_t>(sms / std::max<int64_t>(tiles, 1), kb / 8);
     if (tiles * 2 <= sms && split >= 2) {
-      // fp32 partial-sum workspace: one per (device, stream, extent), zeroed once — the finishing kernel leaves it zeroed
-      static std::map<std::array<int64_t, 4>, at::Tensor> ws_cache;
-      static std::mutex ws_mu;
-      at::Tensor ws;
-      {
-        std::lock_guard<std::mutex> lock(ws_mu);
-        const std::array<int64_t, 4> key{a.device().index(), reinterpret_cast<int64_t>(stream.stream()), M, N};
-        auto it = ws_cache.find(key);
-        if (it == ws_cache.end()) it = ws_cache.emplace(key, at::zeros({M, N}, a.options().dtype(at::kFloat))).first;
-        ws = it->second;
-      }
+      // one fp32 partial per split, written with plain stores and summed in split order by the finishing kernel
+      at::Tensor ws = at::empty({split, M, N}, a.options().dtype(at::kFloat));
       GemmParams q{};
       q.c_f32 = ws.data_ptr<float>();
       q.ldc = N;
       q.alpha = 1.f;
-      q.atomic = 1;
       q.split_k = static_cast<int>(split);
+      q.split_stride = M * N;
       gemm_launch({reinterpret_cast<int64_t>(a.data_ptr())}, a_mn, a.stride(0),
                   {reinterpret_cast<int64_t>(b.data_ptr())}, b_mn, b.stride(0), M, N, K, EPI_F32, q, bn_s, 0, stream);
       const long total = (N % 4 == 0 && p.ldc % 4 == 0) ? M * N / 4 : M * N;
-      const int grid = static_cast<int>(std::min<long>((total + 255) / 256, 148L * 8));
-      splitk_finish_kernel<<<grid, 256, 0, stream>>>(ws.data_ptr<float>(), p.c_bf16, p.ldc, p.bias, p.mask, p.relu ? 1 : 0,
-                                                     p.relu_slope, static_cast<int>(M), static_cast<int>(N));
+      const int grid = static_cast<int>(std::min<long>((total + 255) / 256, sms * 8L));
+      splitk_finish_kernel<<<grid, 256, 0, stream>>>(ws.data_ptr<float>(), M * N, static_cast<int>(split), p.c_bf16, p.ldc,
+                                                     p.bias, p.mask, p.relu ? 1 : 0, p.relu_slope, static_cast<int>(M),
+                                                     static_cast<int>(N));
       C10_CUDA_KERNEL_LAUNCH_CHECK();
       return c;
     }
@@ -338,8 +353,8 @@ at::Tensor gemm_bf16(const at::Tensor& a, bool a_mn, const at::Tensor& b, bool b
   return c;
 }
 
-// out[M,N] fp32 (+)= alpha * Aᵀ-style product; split_k>1 accumulates atomically (out must be pre-zeroed
-// or hold the value to accumulate onto).
+// out[M,N] fp32 (+)= alpha * Aᵀ-style product; split_k > 1 adds the product onto out (which must be pre-zeroed or hold the
+// value to accumulate onto): the splits' partials go to a workspace and are summed in split order.
 void gemm_f32(const at::Tensor& a, bool a_mn, const at::Tensor& b, bool b_mn, at::Tensor out, double alpha,
               bool accumulate, int64_t split_k, int64_t bn) {
   TORCH_CHECK(a.is_cuda() && a.scalar_type() == at::kBFloat16 && b.scalar_type() == at::kBFloat16);
@@ -349,15 +364,29 @@ void gemm_f32(const at::Tensor& a, bool a_mn, const at::Tensor& b, bool b_mn, at
   const int64_t M = a_mn ? a.size(1) : a.size(0), K = a_mn ? a.size(0) : a.size(1);
   const int64_t N = b_mn ? b.size(1) : b.size(0);
   TORCH_CHECK((b_mn ? b.size(0) : b.size(1)) == K && out.size(0) == M && out.size(1) == N, "shape mismatch");
+  auto stream = at::cuda::getCurrentCUDAStream();
+  const int64_t splits = std::max<int64_t>(1, std::min<int64_t>(split_k, (K + BLOCK_K - 1) / BLOCK_K));
   GemmParams p{};
-  p.c_f32 = out.data_ptr<float>();
-  p.ldc = out.stride(0);
   p.alpha = static_cast<float>(alpha);
-  p.split_k = static_cast<int>(split_k);
-  p.atomic = (accumulate || split_k > 1) ? 1 : 0;
+  p.split_k = static_cast<int>(splits);
+  if (splits == 1) {
+    p.c_f32 = out.data_ptr<float>();
+    p.ldc = out.stride(0);
+    p.atomic = accumulate ? 1 : 0;           // one add per element onto the existing value
+    gemm_launch({reinterpret_cast<int64_t>(a.data_ptr())}, a_mn, a.stride(0),
+                {reinterpret_cast<int64_t>(b.data_ptr())}, b_mn, b.stride(0), M, N, K, EPI_F32, p, static_cast<int>(bn), 0,
+                stream);
+    return;
+  }
+  at::Tensor ws = at::empty({splits, M, N}, out.options());
+  p.c_f32 = ws.data_ptr<float>();
+  p.ldc = N;
+  p.split_stride = M * N;
   gemm_launch({reinterpret_cast<int64_t>(a.data_ptr())}, a_mn, a.stride(0),
-              {reinterpret_cast<int64_t>(b.data_ptr())}, b_mn, b.stride(0), M, N, K, EPI_F32, p,
-              static_cast<int>(bn), 0, at::cuda::getCurrentCUDAStream());
+              {reinterpret_cast<int64_t>(b.data_ptr())}, b_mn, b.stride(0), M, N, K, EPI_F32, p, static_cast<int>(bn), 0,
+              stream);
+  splitk_reduce(ws, static_cast<int>(splits), out.data_ptr<float>(), out.stride(0), static_cast<int>(M), static_cast<int>(N),
+                stream);
 }
 
 // The sufficient-factor outer product with the optimizer fused into the epilogue:

@@ -14,7 +14,7 @@ namespace psd {
 // packed pixels leave as one or two 16-byte stores.
 // Threads walk the PHYSICAL output (border and alignment columns included) so the kernel itself writes the zeros —
 // no separate memset pass over the 100 MB activation — with 32-bit indices and magic-number divides (the first
-// version spent ~300 of its ~485 instructions per thread on three 64-bit divisions; ncu: 73 % issue-active).
+// version spent most of its instructions per thread on three 64-bit divisions and was issue-bound).
 template <typename TIn, int CP, int PX>
 __global__ void __launch_bounds__(256)
 transform_kernel(const TIn* __restrict__ x, __nv_bfloat16* __restrict__ out, const int* __restrict__ h_off,
@@ -112,7 +112,7 @@ at::Tensor transform_nhwc(const at::Tensor& x, const at::Tensor& h_off, const at
   const FastDiv d_owg = make_fastdiv(owg), d_ohp = make_fastdiv(OHp);
   auto op = reinterpret_cast<__nv_bfloat16*>(out.data_ptr());
 #define PSD_XF(T, CPV)                                                                                          \
-  transform_kernel<T, CPV, kPx><<<grid_for(total, 256, 148 * 32), 256, 0, stream>>>(                                         \
+  transform_kernel<T, CPV, kPx><<<grid_for(total, 256, 132 * 32), 256, 0, stream>>>(                                         \
       x.data_ptr<T>(), op, h_off.data_ptr<int>(), w_off.data_ptr<int>(), flip.data_ptr<uint8_t>(), mp, mean_mode, \
       static_cast<float>(scale), C, H, W, OH, OW, opad, OWp, d_owg, d_ohp, static_cast<uint32_t>(total), s2d ? 1 : 0)
   if (x.scalar_type() == at::kByte) {
@@ -251,8 +251,10 @@ at::Tensor dropout_apply(const at::Tensor& x, double ratio, int64_t seed, const 
 }
 
 // ------------------------------------------------------------------ bias gradient: out[c] (+)= sum_rows dy[row, c]
+// Pass 1: block (x, y) sums the rows of split y for 64 columns into part[y][c]; pass 2 adds the splits onto out in split
+// order (no atomics: the sum does not depend on which block finishes first).
 __global__ void __launch_bounds__(256)
-colsum_kernel(const __nv_bfloat16* __restrict__ dy, long ld, long rows, int C, float* __restrict__ out, float alpha) {
+colsum_kernel(const __nv_bfloat16* __restrict__ dy, long ld, long rows, int C, float* __restrict__ part) {
   // blockDim = (8 vec-columns, 32 row lanes); grid = (ceil(C/64), row splits)
   __shared__ float red[32][65];
   const int v = threadIdx.x, ry = threadIdx.y;
@@ -277,8 +279,17 @@ colsum_kernel(const __nv_bfloat16* __restrict__ dy, long ld, long rows, int C, f
 #pragma unroll 8
     for (int r = 0; r < 32; ++r) s += red[r][t];
     const int c = blockIdx.x * 64 + t;
-    if (c < C) atomicAdd(out + c, s * alpha);
+    if (c < C) part[static_cast<long>(blockIdx.y) * C + c] = s;
   }
+}
+
+__global__ void __launch_bounds__(256)
+colsum_finish_kernel(const float* __restrict__ part, int splits, int C, float* __restrict__ out, float alpha, int accumulate) {
+  const int c = blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= C) return;
+  float s = 0.f;
+  for (int y = 0; y < splits; ++y) s += part[static_cast<long>(y) * C + c];
+  out[c] = (accumulate ? out[c] : 0.f) + s * alpha;
 }
 
 // dy viewed as [rows, C] with row pitch ld (C % 8 == 0); out fp32 [C] (zeroed unless accumulate).
@@ -287,12 +298,15 @@ void colsum(const at::Tensor& dy, int64_t rows, int64_t C, int64_t ld, at::Tenso
   TORCH_CHECK(C % 8 == 0 && ld % 8 == 0, "colsum: C and pitch must be multiples of 8");
   c10::cuda::CUDAGuard guard(dy.device());
   auto stream = at::cuda::getCurrentCUDAStream();
-  if (!accumulate) C10_CUDA_CHECK(cudaMemsetAsync(out.data_ptr(), 0, C * sizeof(float), stream));
   dim3 block(8, 32);
   const int gx = (C + 63) / 64;
   const int gy = static_cast<int>(std::max<long>(1, std::min<long>((rows + 255) / 256, std::max(1, 592 / gx))));
+  at::Tensor part = at::empty({gy, C}, out.options());
   colsum_kernel<<<dim3(gx, gy), block, 0, stream>>>(reinterpret_cast<const __nv_bfloat16*>(dy.data_ptr()), ld, rows, C,
-                                                    out.data_ptr<float>(), static_cast<float>(alpha));
+                                                    part.data_ptr<float>());
+  C10_CUDA_KERNEL_LAUNCH_CHECK();
+  colsum_finish_kernel<<<(C + 255) / 256, 256, 0, stream>>>(part.data_ptr<float>(), gy, C, out.data_ptr<float>(),
+                                                            static_cast<float>(alpha), accumulate ? 1 : 0);
   C10_CUDA_KERNEL_LAUNCH_CHECK();
 }
 

@@ -121,9 +121,8 @@ lrn_kernel(const __nv_bfloat16* __restrict__ x, const __nv_bfloat16* __restrict_
 // reads the neighbouring 16-byte vectors directly (they are L1 hits: the same lines are being read by the
 // adjacent threads), so there is no shared-memory staging, no bank conflicts and DRAM sees every byte once.
 // Register-resident variant (local_size <= 9): one thread = 8 channels of one pixel, neighbours' vectors loaded
-// directly (the channel window of a pixel is contiguous in NHWC).  ncu showed the first version issue-bound (90 %
-// issue-active, ~405 / ~470 instructions per thread fwd / bwd): 64-bit index divisions, libm log2f/exp2f and 5-tap
-// re-summation.  This version uses a magic-number divide, MUFU lg2/ex2 and sliding-window sums.
+// directly (the channel window of a pixel is contiguous in NHWC).  The first version was issue-bound: 64-bit index
+// divisions, libm log2f/exp2f and 5-tap re-summation.  This version uses a magic-number divide, MUFU lg2/ex2 and sliding-window sums.
 template <int N>
 __device__ __forceinline__ void load_window(const __nv_bfloat16* p, int v, int c8, float (&w)[24]) {
   float t[8];
@@ -222,7 +221,7 @@ static void lrn_launch(bool bwd, const at::Tensor& x, const at::Tensor* dy, at::
   int pix = std::max(1, std::min(64, static_cast<int>((96 * 1024) / (arrays * CP * 4))));
   const size_t smem = static_cast<size_t>(arrays) * pix * CP * sizeof(float);
   auto stream = at::cuda::getCurrentCUDAStream();
-  const int grid = static_cast<int>(std::min<long>((npix + pix - 1) / pix, 148 * 8));
+  const int grid = static_cast<int>(std::min<long>((npix + pix - 1) / pix, 132 * 8));
   long dpitch = 0;
   const __nv_bfloat16* dyp = nullptr;
   if (bwd) {
@@ -235,7 +234,7 @@ static void lrn_launch(bool bwd, const at::Tensor& x, const at::Tensor* dy, at::
   if (size <= 9) {
     const long total = npix * (v.C / 8);
     TORCH_CHECK(total < (1L << 31) && v.pitch < (1L << 31), "lrn: tensor too large for 32-bit indexing");
-    const int g2 = grid_for(total, 256, 148 * 32);
+    const int g2 = grid_for(total, 256, 132 * 32);
     const float aon = static_cast<float>(alpha / size), bt = static_cast<float>(beta);
     const FastDiv dc8 = make_fastdiv(static_cast<uint32_t>(v.C / 8));
     const uint32_t tot = static_cast<uint32_t>(total);

@@ -69,7 +69,7 @@ inline at::Tensor empty_nhwc(int64_t n, int64_t c, int64_t h, int64_t w, const a
   return at::empty({n, c, h, w}, opt.memory_format(at::MemoryFormat::ChannelsLast));
 }
 
-inline int grid_for(long work, int block, int max_blocks = 148 * 16) {
+inline int grid_for(long work, int block, int max_blocks = 132 * 16) {
   long g = (work + block - 1) / block;
   return static_cast<int>(std::max<long>(1, std::min<long>(g, max_blocks)));
 }

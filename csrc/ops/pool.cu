@@ -17,8 +17,7 @@ struct PoolGeom {
   FastDiv d_c8, d_ow, d_oh, d_w, d_h, d_sh, d_sw;
 };
 
-// ncu showed the first versions of these kernels issue-bound (70-78 % issue-active; ~760 instructions per thread for the
-// 3x3 forward, ~500 for the backward): 64-bit index divisions and per-channel fp32 compare/select chains.  Now: 32-bit
+// The first versions of these kernels were issue-bound: 64-bit index divisions and per-channel fp32 compare/select chains.  Now: 32-bit
 // indices with magic-number divides, MAX forward entirely in packed bf16x2 (max + compare-mask + one LOP3 per channel
 // pair and tap; bf16 compares are exact, so the result equals the fp32 computation), MAX backward with SIMD byte compares.
 
@@ -236,7 +235,7 @@ std::tuple<at::Tensor, at::Tensor> pool_fwd(const at::Tensor& x, bool is_max, at
   auto xp = reinterpret_cast<const __nv_bfloat16*>(x.data_ptr());
   auto yp = reinterpret_cast<__nv_bfloat16*>(y.data_ptr());
   uint8_t* ip = idx.defined() ? idx.data_ptr<uint8_t>() : nullptr;
-  const int grid = grid_for(total, 256, 148 * 32);
+  const int grid = grid_for(total, 256, 132 * 32);
   const int kt = (g.kh == g.kw && (g.kh == 2 || g.kh == 3)) ? g.kh : 0;
 #define PSD_PF(MX, KT) pool_fwd_kernel<MX, KT><<<grid, 256, 0, stream>>>(xp, yp, MX ? ip : nullptr, g, static_cast<uint32_t>(total))
   if (is_max) { if (kt == 3) PSD_PF(true, 3); else if (kt == 2) PSD_PF(true, 2); else PSD_PF(true, 0); }
@@ -259,7 +258,7 @@ at::Tensor pool_bwd(const at::Tensor& dy, const at::Tensor& idx, bool is_max, at
   auto stream = at::cuda::getCurrentCUDAStream();
   auto dyp = reinterpret_cast<const __nv_bfloat16*>(dy.data_ptr());
   auto dxp = reinterpret_cast<__nv_bfloat16*>(dx.data_ptr());
-  const int grid = grid_for(total, 256, 148 * 32);
+  const int grid = grid_for(total, 256, 132 * 32);
   const int ncand = std::max((g.kh + g.sh - 1) / g.sh, (g.kw + g.sw - 1) / g.sw);
   const int nc = ncand <= 3 ? ncand : 0;
   const uint8_t* ip = nullptr;

@@ -144,7 +144,7 @@ static void launch_softmax(const at::Tensor& a, const at::Tensor* b, at::Tensor&
     const int grid = grid_for(va.rows * 32, 256);
     softmax_rows_kernel<BWD><<<grid, 256, 0, st>>>(ap, bp, op, va.rows, va.C, va.ld, vb.ld, vo.ld);
   } else {
-    const int grid = static_cast<int>(std::min<long>(va.rows, 148L * 8));
+    const int grid = static_cast<int>(std::min<long>(va.rows, 132L * 8));
     softmax_long_kernel<BWD><<<grid, 256, 0, st>>>(ap, bp, op, va.rows, va.C, va.ld, vb.ld, vo.ld);
   }
   C10_CUDA_KERNEL_LAUNCH_CHECK();

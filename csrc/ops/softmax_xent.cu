@@ -31,7 +31,7 @@ __device__ __forceinline__ float to_f<__nv_bfloat16>(__nv_bfloat16 v) { return _
 template <typename T>
 __global__ void __launch_bounds__(256)
 softmax_xent_kernel(const T* __restrict__ x, long ldx, const float* __restrict__ label, T* __restrict__ dx, long lddx,
-                    float* __restrict__ prob, float* __restrict__ loss, int rows, int C, float grad_scale) {
+                    float* __restrict__ prob, float* __restrict__ row_loss, int rows, int C, float grad_scale) {
   __shared__ float red[8];
   __shared__ float bc;
   const int row = blockIdx.x;
@@ -72,8 +72,24 @@ softmax_xent_kernel(const T* __restrict__ x, long ldx, const float* __restrict__
       if constexpr (sizeof(T) == 2) dx[static_cast<long>(row) * lddx + c] = __float2bfloat16(g);
       else dx[static_cast<long>(row) * lddx + c] = g;
     }
-    if (c == lab) atomicAdd(loss, -__logf(fmaxf(p, 1.17549435e-38f)) / static_cast<float>(rows));
+    if (c == lab) row_loss[row] = -__logf(fmaxf(p, 1.17549435e-38f));
   }
+}
+
+// loss = mean of the per-row losses, summed in a fixed order (strided per thread, then a fixed tree): no atomics, so the
+// loss is the same in every run.
+__global__ void __launch_bounds__(256)
+mean_rows_kernel(const float* __restrict__ row_loss, int rows, float* __restrict__ loss) {
+  __shared__ float red[256];
+  float s = 0.f;
+  for (int r = threadIdx.x; r < rows; r += blockDim.x) s += row_loss[r];
+  red[threadIdx.x] = s;
+  __syncthreads();
+  for (int w = blockDim.x / 2; w > 0; w >>= 1) {
+    if (threadIdx.x < w) red[threadIdx.x] += red[threadIdx.x + w];
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) loss[0] = red[0] / static_cast<float>(rows);
 }
 
 // x: [rows, C] (bf16 or fp32), label: [rows] fp32 class ids.  Returns (loss[1] fp32, dx like x, prob fp32 or empty).
@@ -83,7 +99,8 @@ std::tuple<at::Tensor, at::Tensor, at::Tensor> softmax_xent(const at::Tensor& x,
   TORCH_CHECK(label.scalar_type() == at::kFloat && label.numel() == x.size(0) && label.is_contiguous());
   c10::cuda::CUDAGuard guard(x.device());
   const int rows = x.size(0), C = x.size(1);
-  at::Tensor loss = at::zeros({1}, x.options().dtype(at::kFloat));
+  at::Tensor loss = at::empty({1}, x.options().dtype(at::kFloat));
+  at::Tensor row_loss = at::zeros({rows}, x.options().dtype(at::kFloat));   // rows whose label is out of range add 0
   at::Tensor dx = want_grad ? at::empty({rows, C}, x.options()) : at::Tensor();
   at::Tensor prob = want_prob ? at::empty({rows, C}, x.options().dtype(at::kFloat)) : at::Tensor();
   auto stream = at::cuda::getCurrentCUDAStream();
@@ -91,14 +108,16 @@ std::tuple<at::Tensor, at::Tensor, at::Tensor> softmax_xent(const at::Tensor& x,
   if (x.scalar_type() == at::kBFloat16) {
     softmax_xent_kernel<__nv_bfloat16><<<rows, 256, 0, stream>>>(
         reinterpret_cast<const __nv_bfloat16*>(x.data_ptr()), x.stride(0), label.data_ptr<float>(),
-        want_grad ? reinterpret_cast<__nv_bfloat16*>(dx.data_ptr()) : nullptr, C, pp, loss.data_ptr<float>(), rows, C,
+        want_grad ? reinterpret_cast<__nv_bfloat16*>(dx.data_ptr()) : nullptr, C, pp, row_loss.data_ptr<float>(), rows, C,
         static_cast<float>(grad_scale));
   } else {
     TORCH_CHECK(x.scalar_type() == at::kFloat, "softmax_xent: bf16 or fp32 logits");
     softmax_xent_kernel<float><<<rows, 256, 0, stream>>>(x.data_ptr<float>(), x.stride(0), label.data_ptr<float>(),
                                                          want_grad ? dx.data_ptr<float>() : nullptr, C, pp,
-                                                         loss.data_ptr<float>(), rows, C, static_cast<float>(grad_scale));
+                                                         row_loss.data_ptr<float>(), rows, C, static_cast<float>(grad_scale));
   }
+  C10_CUDA_KERNEL_LAUNCH_CHECK();
+  mean_rows_kernel<<<1, 256, 0, stream>>>(row_loss.data_ptr<float>(), rows, loss.data_ptr<float>());
   C10_CUDA_KERNEL_LAUNCH_CHECK();
   return {loss, want_grad ? dx : at::empty({0}, x.options()), want_prob ? prob : at::empty({0}, x.options())};
 }

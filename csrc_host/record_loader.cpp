@@ -2,8 +2,8 @@
 //
 // The reference's data path is C++ end to end: a LevelDB/LMDB cursor, Datum::ParseFromString and the
 // DataTransformer run on one prefetch thread per data layer (src/caffe/layers/data_layer.cpp:143-259,
-// src/caffe/layers/base_data_layer.cpp:57-104).  A B200 consumes > 50 k ImageNet-sized records per second, i.e.
-// > 10 GB/s of record payload, which a single thread (let alone Python) cannot decode, so this module
+// src/caffe/layers/base_data_layer.cpp:57-104).  One H100 trains AlexNet at ~47 k ImageNet-sized records per second, i.e.
+// ~7 GB/s of record payload, which a single thread (let alone Python) cannot decode, so this module
 //   * memory-maps the PDB record file (b"PDB1" | u64 n | n x (u32 klen, u32 vlen, key, value)) and indexes it once,
 //   * parses the Datum wire format in place (no protobuf library, no copies other than the payload memcpy),
 //   * fills caller-owned batch buffers (page-locked memory handed in from PyTorch) with a pool of worker threads, and

@@ -1,7 +1,7 @@
 """poseidon_b200 — a Blackwell-native distributed CNN training engine with the capabilities
 of petuum/poseidon (PMLS-Caffe): Caffe prototxt / caffemodel / solverstate compatible,
 distributed wait-free backprop + sufficient-factor broadcasting re-imagined as fused
-sm_100a CUDA kernels over NVLink 5 / NVSwitch.  See SURVEY.md / DESIGN.md.
+sm_90a CUDA kernels over NVLink / NVSwitch.  See SURVEY.md / DESIGN.md.
 """
 __version__ = "0.1.0"
 

@@ -1,7 +1,7 @@
 """Branch-parallel execution: independent branches of the layer graph run on separate CUDA streams ("lanes").
 
 GoogLeNet's inception modules fan one blob out to four branches of small convolutions (at batch 32 a 14x14 stage has
-49 m-blocks, a 7x7 stage 13 — a fraction of the 148 SMs), plus two auxiliary classifier heads hanging off the trunk.
+49 m-blocks, a 7x7 stage 13 — a fraction of the 132 SMs), plus two auxiliary classifier heads hanging off the trunk.
 Run back to back every one of those kernels leaves most of the chip idle; on separate streams the branches overlap, and
 the whole-step CUDA graph records them as parallel branches.  The reference executes layers strictly in sequence
 (src/caffe/net.cpp:709-750 ForwardFromTo; :752-784 BackwardFromTo) — one kernel at a time on one stream.

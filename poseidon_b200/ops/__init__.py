@@ -1,7 +1,7 @@
 """Op namespaces.  ``get(ctx)`` returns the engine a layer should call into:
 
 * ``torch``  – :mod:`.torch_engine` (CPU, or cuDNN/cuBLAS through PyTorch: the baseline)
-* ``sm100``  – :mod:`.sm100` (hand-written sm_100a CUDA kernels; requires a B200)
+* ``sm100``  – :mod:`.sm100` (hand-written sm_90a CUDA kernels; requires an H100)
 """
 from __future__ import annotations
 

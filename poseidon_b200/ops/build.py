@@ -1,7 +1,7 @@
-"""Build / load the sm_100a CUDA extension (in-tree, so the .so travels with the repo).
+"""Build / load the sm_90a CUDA extension (in-tree, so the .so travels with the repo).
 
 All kernels live in ``csrc/`` and are compiled with
-``-gencode arch=compute_100a,code=sm_100a -lineinfo`` into ``poseidon_b200/_ext/poseidon_b200_C.so``;
+``-gencode arch=compute_90a,code=sm_90a -lineinfo`` into ``poseidon_b200/_ext/poseidon_b200_C.so``;
 ops register themselves under ``torch.ops.poseidon``.
 """
 from __future__ import annotations
@@ -20,7 +20,7 @@ _lock = threading.Lock()
 _loaded = False
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "--expt-relaxed-constexpr", "-Xptxas", "-v", "--threads", "4",
     "-DPSD_SPIN_LIMIT=67108864u",
 ]

@@ -3,12 +3,12 @@
 Why: the sm100 engine is two things — the CUDA kernels in ``csrc/`` and a fair amount of Python around them that decides
 operand layouts (ROW / space-to-depth / 8-channel first layers, channel-padded K, (h, w, c) inner-product weights), keeps
 bf16 shadows in step with fp32 masters, plans epilogue fusion and routes gradients into the optimizer kernels.  The kernels
-can only be tested on a B200; the Python around them is just as easy to break, and with ``POSEIDON_EMULATE=1`` it runs on
+can only be tested on an H100; the Python around them is just as easy to break, and with ``POSEIDON_EMULATE=1`` it runs on
 any machine: ``sm100.K()`` hands out this module's :class:`EmulatedKernels` instead of the compiled extension, and the
 whole engine (``Solver(engine="sm100")``, fusion plan, FusedBackend's single-process path) steps on the CPU.
 
 Every method documents the layout contract of the kernel it stands in for (file:line of the CUDA implementation); the
-arithmetic is fp32 with one bf16 rounding at the output, which is also what the kernels do (fp32 accumulation in TMEM,
+arithmetic is fp32 with one bf16 rounding at the output, which is also what the kernels do (fp32 accumulation in registers,
 bf16 store), so results agree with the GPU to bf16 rounding.  This is a *test double*: it is never selected implicitly,
 it is slow.  The multi-GPU peer-memory ops run too: ranks are processes, the symmetric arena is host shared memory
 (:class:`EmulatedArena`), the flag protocol is the kernels'.

@@ -1,7 +1,7 @@
 """Plain-PyTorch implementations of every Caffe op with Caffe's exact semantics.
 
 These serve three purposes: (1) the CPU path (LeNet plumbing config), (2) the
-"vendor" GPU baseline (cuDNN/cuBLAS through PyTorch) that the sm_100a kernels are
+"vendor" GPU baseline (cuDNN/cuBLAS through PyTorch) that the sm_90a kernels are
 measured against, (3) the fp32 numerical oracle for every hand-written CUDA kernel.
 
 Semantics follow SURVEY.md Appendix A; file:line citations are on each function.

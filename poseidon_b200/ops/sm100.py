@@ -1,4 +1,4 @@
-"""The sm100 engine: every hot op runs a hand-written sm_100a kernel from ``csrc/``.
+"""The sm100 engine: every hot op runs a hand-written sm_90a kernel from ``csrc/``.
 
 Conventions
 -----------
@@ -60,7 +60,7 @@ def K():
         else:
             load_extension()
             _ops = CountingOps(torch.ops.poseidon)
-            # schedule switches (defaults are the measured best; see profiles/r2_conv_ncu_summary.md)
+            # schedule switches (A/B knobs; the defaults are what the kernels ship with)
             env = os.environ
             if "POSEIDON_PAIR_CTA" in env:
                 torch.ops.poseidon.set_pair_cta(int(env["POSEIDON_PAIR_CTA"]))
@@ -164,8 +164,8 @@ class ConvState:
         # most a third of the MMA work; the TMA zero-fills the extra slots, the weight operand carries zeros there.
         self.cgk = self.cg            # K slots per tap of the fprop / wgrad operand
         self.cok = self.Cout // self.groups      # K slots per tap of the dgrad operand
-        # Opt-in (POSEIDON_PAD_K=1): numerically validated on B200, but AlexNet throughput was unchanged (conv2: a third
-        # more MMA work bought back by the cheaper producer: 78.9 k vs 80.0 k img/s) and GoogLeNet is not yet measured.
+        # Opt-in (POSEIDON_PAD_K=1): numerically validated (tests/test_zz_padded_channels_gpu.py); its effect on throughput is
+        # not measured on H100.
         if not self.row_mode and os.environ.get("POSEIDON_PAD_K", "0") == "1":
             self.cgk = _pad64(self.cg)
             self.cok = _pad64(self.Cout // self.groups)
@@ -186,8 +186,8 @@ class ConvState:
     def _try_s2d(self, layer):
         """Stride-4 first layers (AlexNet / CaffeNet conv1): space-to-depth by 4 turns the 11x11/s4 convolution over
         4 (padded) channels into a 3x3/s1 convolution over 4*4*4 = 64 channels — a plain TAP-mode implicit GEMM whose
-        operand the TMA engine fetches in im2col mode, instead of the cp.async ROW gather (conv1 fprop 300 us -> see
-        profiles/).  The data layer's transform kernel writes the s2d layout directly."""
+        operand the TMA engine fetches in im2col mode, instead of the cp.async ROW gather.  The data layer's transform
+        kernel writes the s2d layout directly."""
         if os.environ.get("POSEIDON_S2D", "1") == "0" or tuple(layer.stride) != (4, 4) or layer.pad[0] != layer.pad[1]:
             return
         in_hw = getattr(layer, "in_hw", None)
@@ -546,7 +546,7 @@ def _strided_dgrad(k, st: "ConvState", layer, dy: torch.Tensor, xin: torch.Tenso
     Input row ih = a + sh * i' (phase a) only receives taps r = r0 + sh * j with r0 = (a + ph) mod sh, and then
         oh = (ih + ph - r) / sh = i' + q - j,          q = (a + ph - r0) / sh   (an integer >= 0),
     i.e. the pixels of one phase are a stride-1 data gradient over dY with the sub-filter W[:, :, r0::sh, s0::sw] and
-    padding (q_h, q_w): the same tcgen05 dgrad kernel, one launch per phase, each writing one interleaved sub-grid of dX.
+    padding (q_h, q_w): the same wgmma dgrad kernel, one launch per phase, each writing one interleaved sub-grid of dX.
     No atomics, no col2im scatter."""
     sh, sw = layer.stride
     ph, pw = layer.pad

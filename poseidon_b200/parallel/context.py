@@ -114,7 +114,7 @@ def init_rank_context(device: Optional[str] = None, hostfile: Optional[str] = No
         # NumaMgr's role (ps/src/petuum_ps/thread/numa_mgr.hpp:28-203): the per-GPU process — and with it the first-touch
         # placement of its pinned input buffers — stays on the CPUs of the GPU's NUMA node, so the per-step H2D copies do
         # not cross sockets.  POSEIDON_NUMA=off (default, like the reference's optional NumaMgr) | center | even;
-        # measured neutral on a 2-GPU / 2-socket allocation (profiles/r2_numa_2gpu_call25.log), not measured at 8 GPUs.
+        # its effect is not measured on H100.
         policy = os.environ.get("POSEIDON_NUMA", "off")
         if policy != "off":
             from ..utils.affinity import pin_to_gpu_numa

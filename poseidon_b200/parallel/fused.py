@@ -11,8 +11,8 @@
 * ``FusedBackend`` — per-bucket ``allreduce_sgd`` kernel (two-shot, history sharded across ranks;
   one-shot for small buckets) launched from the DWBP hooks on a high-priority stream.
 * ``FusedSFB`` — sufficient-factor broadcasting: every rank PUSHES its u, v into slot `rank` of every peer's arena
-  (one NVSwitch-multicast store stream) and raises a release flag; ONE tcgen05 kernel then walks the P local slots as
-  P reduction sources (waiting on slot p's flag right before its first TMA load) and accumulates Σ_p u_pᵀ v_p in TMEM
+  (one NVSwitch-multicast store stream) and raises a release flag; ONE wgmma kernel then walks the P local slots as
+  P reduction sources (waiting on slot p's flag right before its first TMA load) and accumulates Σ_p u_pᵀ v_p in registers
   with the optimizer step fused into its epilogue — no dense ΔW ever exists, locally or on the wire.  With one rank it
   degenerates to the fused wgrad+update kernel.
 
@@ -169,8 +169,8 @@ class FusedBackend(Backend):
         self.use_multimem = use_multimem and os.environ.get("POSEIDON_MULTIMEM", "1") != "0"
         # SFB reconstruct: optimizer step fused into the outer-product kernel's epilogue (1), or the two-pass form
         # "P-source outer product -> fp32 buffer (bulk row stores), then the streaming update kernel" (0)
-        # Measured on 2 x B200 (profiles/r2_scale2_call56.log): two-pass 3.339 ms / step, fused epilogue 3.447 ms (1 GPU on the
-        # same box: 3.280 ms) — the epilogue's W/H stream runs at 37 % of the HBM copy rate, the update kernel at 96-100 %.
+        # The two-pass form is the default: the update kernel streams W / H as one linear pass, the epilogue touches them
+        # tile by tile.
         self.fuse_sfb_sgd = os.environ.get("POSEIDON_SFB_FUSED_SGD", "0") == "1"
         self.arena: Optional[SymmetricArena] = None
         self.epoch = 0
@@ -222,7 +222,7 @@ class FusedBackend(Backend):
                 if isinstance(st, sm100.ConvState) and not st.row_mode and layer.weight.requires_grad:
                     layer._grad_sink = self
         self.multi_update = self.world == 1 and os.environ.get("POSEIDON_MULTI_UPDATE", "1") != "0"
-        # (measured neutral on AlexNet / VGG-16, profiles/r2_side_stream_call26.log: off by default)
+        # (off by default)
         self._early_ip_update = os.environ.get("POSEIDON_EARLY_IP_UPDATE", "0") == "1"
         self._deferred = []
         self.per_worker_state = self.ssp and self.world > 1
@@ -728,7 +728,7 @@ class FusedSFB:
     Staging layout inside every rank's arena (single-buffered; a rank may only overwrite a peer's slot after that peer
     raised its *consumed* flag for the previous step):  U[P][M][N], V[P][M][K] bf16.  Rank r
     *pushes* its factors into slot r of every rank (one NVSwitch-multicast store stream, or P2P stores),
-    raises its epoch flag on every peer, and the tcgen05 kernel walks the P slots as P reduction sources,
+    raises its epoch flag on every peer, and the wgmma kernel walks the P slots as P reduction sources,
     waiting on slot p's flag right before its first TMA load of that slot — so the outer product of the
     factors that have already landed overlaps the arrival of the rest.  All ranks reduce in the same slot
     order, so replicas stay bit-identical."""

@@ -10,7 +10,7 @@ This file holds the library-based implementation (``all_gather`` + cuBLAS GEMM) 
 baseline engine and by the CPU/gloo tests, plus the cost-model hybrid chooser that decides
 per layer between SFB and dense all-reduce (absent from the reference, which applies SFB to
 every IP weight whenever ``--svb`` is on: tools/caffe_main.cpp:149-151, solver.cpp:434-436).
-The fused NVLink-multicast + tcgen05 kernel version lives in ``fused.py`` / ``csrc/comm``.
+The fused NVLink-multicast + wgmma kernel version lives in ``fused.py`` / ``csrc/comm``.
 
 reference: src/caffe/solver.cpp:477-531 (ThreadSyncWithSVB), src/caffe/svb_worker.cpp:125-167,
 src/caffe/layers/inner_product_layer.cu:55-64 (ComputeGradientFromSV_gpu),

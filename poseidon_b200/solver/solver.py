@@ -254,7 +254,7 @@ class Solver:
         if self.engine == "sm100" and comm in ("fused", "local"):
             from ..ops import sm100
             if not sm100.active(self.device):
-                raise RuntimeError("the sm100 engine needs a CUDA device (B200)")
+                raise RuntimeError("the sm100 engine needs a CUDA device (H100)")
             from ..parallel.fused import FusedBackend
             self.comm_name = "fused"
             backend = FusedBackend(self.svb, sfb_mode, grad_reduce, staleness=self.staleness)

@@ -8,7 +8,7 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: test needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: test needs a CUDA device (run on an H100)")
     config.addinivalue_line("markers", "multigpu: test needs >= 2 CUDA devices")
 
 
@@ -25,7 +25,7 @@ def pytest_collection_modifyitems(config, items):
 
 @pytest.fixture(scope="session")
 def ext():
-    """The in-tree sm_100a extension; GPU tests fail loudly if it cannot be loaded."""
+    """The in-tree sm_90a extension; GPU tests fail loudly if it cannot be loaded."""
     from poseidon_b200.ops import build
     build.load_extension()
     import torch

@@ -1,4 +1,4 @@
-"""Multi-GPU (>= 2 B200) checks of the fused NVLink backend: in-kernel all-reduce + optimizer, fused SFB,
+"""Multi-GPU (>= 2 H100) checks of the fused NVLink backend: in-kernel all-reduce + optimizer, fused SFB,
 against single-GPU training on the concatenated batch; plus the NCCL baseline."""
 import numpy as np
 import pytest

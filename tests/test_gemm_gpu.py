@@ -1,4 +1,4 @@
-"""tcgen05 GEMM family vs fp32 PyTorch references (run on B200)."""
+"""wgmma GEMM family vs fp32 PyTorch references (run on an H100)."""
 import pytest
 import torch
 

@@ -1,5 +1,5 @@
 """Round-2 layer kernels (sigmoid / tanh / absval / bnll / power / threshold, eltwise, channel softmax, MVN, within-channel
-LRN, stochastic pooling) against the fp32 oracle in ops/reference.py — forward and backward, on a B200."""
+LRN, stochastic pooling) against the fp32 oracle in ops/reference.py — forward and backward, on an H100."""
 import pytest
 import torch
 

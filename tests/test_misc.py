@@ -158,11 +158,9 @@ def test_caffe_root_placeholder_and_relative_paths(tmp_path, monkeypatch):
 def test_reference_example_solvers_load_unmodified():
     """examples/mnist + examples/cifar10 solver files of the reference (CAFFE_ROOT placeholders included) build nets."""
     import os
-    import pytest
     from poseidon_b200 import get_solver, proto as P
-    ref = "/root/reference/examples"
-    if not os.path.isdir(ref):
-        pytest.skip("reference tree not mounted")
+    golden =os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "reference")   # the reference's prototxt files
+    ref = os.path.join(golden, "examples")
     for rel in ("mnist/lenet_solver.prototxt", "cifar10/cifar10_quick_solver.prototxt"):
         sp = P.read_solver(os.path.join(ref, rel))
         sp.snapshot, sp.snapshot_after_train, sp.display, sp.test_interval, sp.max_iter = 0, False, 0, 0, 1
@@ -184,13 +182,13 @@ def test_reference_example_solvers_load_unmodified():
         assert tuple(out[top].shape) == shape, rel
         net.close()
     # models/: POSEIDON_ROOT placeholders in net:, source:, mean_file:, snapshot_prefix: (built, not stepped: batch 256)
-    mref = "/root/reference/models/bvlc_alexnet/solver.prototxt"
+    mref = os.path.join(golden, "models/bvlc_alexnet/solver.prototxt")
     s = get_solver(P.read_solver(mref), engine="torch", model_dir=os.path.dirname(mref))
     assert s.net.layer_by_name["fc8"].weight.shape == (1000, 4096)
     assert "POSEIDON_ROOT" not in s._snapshot_prefix.__func__(type("S", (), {"param": s.param, "model_dir": s.model_dir, "snapshot_dir": "/tmp"})())
     s.close()
-    for mref, n_ip in (("/root/reference/models/bvlc_googlenet/quick_solver.prototxt", 5),
-                       ("/root/reference/models/bvlc_reference_caffenet/solver.prototxt", 3)):
+    for mref, n_ip in ((os.path.join(golden, "models/bvlc_googlenet/quick_solver.prototxt"), 5),
+                       (os.path.join(golden, "models/bvlc_reference_caffenet/solver.prototxt"), 3)):
         s = get_solver(P.read_solver(mref), engine="torch", model_dir=os.path.dirname(mref))
         assert sum(1 for l in s.net.layers if l.type_name == "INNER_PRODUCT") == n_ip and len(s.test_nets) == 1
         s.close()

@@ -1,4 +1,4 @@
-"""sm_100a layer kernels vs fp32 PyTorch references with Caffe semantics (run on B200)."""
+"""sm_90a layer kernels vs fp32 PyTorch references with Caffe semantics (run on an H100)."""
 import pytest
 import torch
 

@@ -1,7 +1,7 @@
-"""Paired-CTA (cta_group::2) kernels vs the single-CTA kernels and the fp32 reference (run on B200).
+"""CTA-pair kernels (2-CTA clusters sharing the B tile by multicast) vs the single-CTA kernels and the fp32 reference.
 
-Every GEMM-shaped op is run twice — ``set_pair_cta(1)`` (default: two CTAs per 256 x BN UMMA, each staging half of B) and
-``set_pair_cta(0)`` (one CTA per 128 x BN UMMA) — on shapes with odd m-block counts (phantom block in the last pair),
+Every GEMM-shaped op is run twice — ``set_pair_cta(1)`` (default: two CTAs per B tile, each fetching half of it for both) and
+``set_pair_cta(0)`` (one CTA per 128 x BN tile) — on shapes with odd m-block counts (phantom block in the last pair),
 ragged edges, split-K, multi-source reductions and the im2col-TMA convolution modes."""
 import pytest
 import torch
@@ -186,7 +186,8 @@ def test_bf16_bulk_epilogue_matches_walk(ext, mode, M, N, K, ldc_pad, bn):
 
 
 def test_pair_gemm_throughput(ext):
-    """8192^3 bf16: paired CTAs vs single-CTA vs cuBLAS on the same box (printed; asserts only a sanity floor)."""
+    """8192^3 bf16: CTA pairs vs single-CTA vs cuBLAS on the same box (printed; asserts a sanity floor relative to cuBLAS on
+    the same card, because the absolute rate of an H100 depends on its power limit)."""
     a, b = _rand((8192, 8192), 1.0, 1), _rand((8192, 8192), 1.0, 2)
     out = torch.empty(8192, 8192, device="cuda", dtype=torch.bfloat16)
 
@@ -208,4 +209,4 @@ def test_pair_gemm_throughput(ext):
     ext.set_pair_cta(1)
     tfc = bench(lambda: torch.matmul(a, b.t()))
     print(f"\n8192^3 bf16: pair {tf2:.0f} TFLOP/s, single-CTA {tf1:.0f}, cuBLAS {tfc:.0f}")
-    assert tf2 > 500
+    assert tf2 > 0.7 * tfc, (tf2, tfc)

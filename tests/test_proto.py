@@ -8,7 +8,7 @@ import pytest
 from poseidon_b200 import proto as P
 from poseidon_b200.proto import parse_text, to_text
 
-REF = "/root/reference"
+REF = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "reference")   # the reference's prototxt files
 
 
 def test_text_roundtrip_and_defaults():
@@ -80,7 +80,6 @@ def test_negative_int_and_int64():
     assert P.BlobProto.FromString(b.SerializeToString()).global_id == -7
 
 
-@pytest.mark.skipif(not os.path.isdir(REF), reason="reference tree not mounted")
 def test_parse_every_reference_prototxt():
     files = glob.glob(REF + "/models/*/*.prototxt") + glob.glob(REF + "/examples/*/*.prototxt")
     assert len(files) >= 20

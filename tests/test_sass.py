@@ -1,6 +1,6 @@
-"""The in-tree extension really is Blackwell-native: `cuobjdump -sass` of the built .so (no GPU needed) must show the
-tcgen05 / TMA / multimem instruction families in the kernels that claim them — and no legacy `mma.sync` (HMMA) anywhere.
-    tcgen05.mma -> UTCHMMA (.2CTA for cta_group::2), tcgen05.ld -> LDTM, TMA tile / im2col loads -> UTMALDG (.IM2COL),
+"""The in-tree extension really is Hopper-native: `cuobjdump -sass` of the built .so (no GPU needed) must show the
+wgmma / TMA / multimem instruction families in the kernels that claim them — and no legacy `mma.sync` (HMMA) anywhere.
+    wgmma.mma_async -> HGMMA, TMA tile / im2col loads -> UTMALDG (.IM2COL, .MULTICAST for cluster-shared tiles),
     bulk async stores -> UBLKCP, multimem.ld_reduce -> LDGMC.E.ADD (multimem.st is a system-scope STG to the multicast address)."""
 import os
 import re
@@ -33,18 +33,17 @@ def _kernels(sass, needle):
     return {k: v for k, v in sass.items() if needle in k}
 
 
-def test_gemm_core_uses_tcgen05_tma_and_tmem(sass):
-    gemm = _kernels(sass, "umma_gemm_kernel")
+def test_gemm_core_uses_wgmma_and_tma(sass):
+    gemm = _kernels(sass, "wgmma_gemm_kernel")
     assert len(gemm) >= 40, len(gemm)
     for name, text in gemm.items():
-        assert "UTCHMMA" in text, f"no tcgen05.mma in {name}"
-        assert "LDTM" in text, f"no tcgen05.ld in {name}"
+        assert re.search(r"HGMMA\.64x\d+x16\.F32\.BF16", text), f"no wgmma in {name}"
         assert "UTMALDG" in text, f"no TMA load in {name}"
-        assert "HMMA" not in text.replace("UTCHMMA", ""), f"legacy mma.sync in {name}"
-    assert any("UTCHMMA.2CTA" in t for t in gemm.values()), "no cta_group::2 MMA"
+        assert not re.search(r"\bHMMA", text), f"legacy mma.sync in {name}"
+    assert any("HGMMA.64x256x16" in t for t in gemm.values()), "no 256-wide wgmma tile"
+    assert any("UTMALDG.2D.MULTICAST" in t for t in gemm.values()), "no CTA-pair multicast of the B tile"
     assert any(re.search(r"UTMALDG\.\dD\.IM2COL", t) for t in gemm.values()), "no im2col-mode TMA"
-    paired_im2col = [t for t in gemm.values() if re.search(r"UTMALDG[.\w]*IM2COL[.\w]*2CTA|UTMALDG[.\w]*2CTA[.\w]*IM2COL", t)]
-    assert paired_im2col, "no paired-CTA im2col loads"
+    assert any("UTMALDG.4D.IM2COL.MULTICAST" in t for t in gemm.values()), "no cluster-shared im2col loads"
     assert any("UBLKCP" in t for t in gemm.values()), "no bulk-async row stores in any epilogue"
 
 

@@ -3,7 +3,7 @@
 ``ops/emulate.py`` stands in for the CUDA kernels (same op surface, same operand layouts), so everything AROUND the
 kernels runs here: operand layouts per first-layer mode, bf16 shadows vs fp32 masters, the epilogue-fusion plan, the
 single-process FusedBackend path, (h, w, c) inner-product weights and their checkpoint conversion.  The kernels
-themselves are tested on a B200 (tests/test_ops_gpu.py, test_engine_gpu.py)."""
+themselves are tested on an H100 (tests/test_ops_gpu.py, test_engine_gpu.py)."""
 import numpy as np
 import pytest
 import torch

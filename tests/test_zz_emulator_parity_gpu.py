@@ -1,7 +1,6 @@
 """The CPU emulation of the op surface (ops/emulate.py) against the kernels it stands in for, op by op, same inputs.
 
 The CPU suite trusts the emulator to test the Python side of the engine; this is the check of the emulator itself.
-(Green on a B200 since round 1's driver run; the provisional xfail marker is gone.)
 Not compared: dropout (the emulation draws its keep-map from a generator instead of the kernel's integer hash)
 and the pooling index tensor (opaque to the caller; only y and dx are contract)."""
 import pytest

@@ -2,7 +2,7 @@
 
 The engine zero-pads such layers to multiples of 8 around the kernels (ops/sm100.py: ConvState.Coutp / Cp, IPState.Kp);
 the Python side of that is covered on the CPU by tests/test_sm100_emulated.py.  These are the same comparisons against the
-fp32 engine on the real kernels.  (File name: collected last, after the suites that were already green on a B200.)"""
+fp32 engine on the real kernels.  (File name: collected last, after the other GPU suites.)"""
 import numpy as np
 import pytest
 import torch
@@ -10,7 +10,6 @@ import torch
 from smallnet import feed, make_data, small_solver_param
 from test_sm100_emulated import _odd_channel_net
 
-# (Green on a B200 since round 1's driver run and round 2's call 1: the provisional xfail marker is gone.)
 pytestmark = [pytest.mark.gpu]
 
 
