@@ -57,8 +57,9 @@ __device__ __forceinline__ uint2 pack_bf16x4(float4 v) {
 }
 
 // ------------------------------------------------------------------------------------ single GPU
-// REARM: the gradient buffer is a persistent accumulation target (conv wgrad adds into it with split-K atomics): leave it
-// zeroed for the next step instead of paying a memset launch per layer and step.
+// REARM: the gradient buffer is a persistent accumulation target (conv wgrad adds onto it: one atomic add per element, or
+// the split-K partials summed in split order): leave it zeroed for the next step instead of paying a memset launch per layer
+// and step.
 template <bool REARM>
 __global__ void __launch_bounds__(256)
 fused_update_kernel(float* __restrict__ w, float* __restrict__ g, float* __restrict__ h, __nv_bfloat16* __restrict__ wb,

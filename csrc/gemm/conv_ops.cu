@@ -26,7 +26,8 @@ void encode_tmap_bf16_3d(CUtensorMap* map, const void* base, int64_t d0, int64_t
                          int box0, int box1, int box2);
 void encode_tmap_im2col_bf16(CUtensorMap* map, const void* base, int64_t C, int64_t W, int64_t H, int64_t N, int64_t pitch,
                              int lower_w, int lower_h, int upper_w, int upper_h, int pixels, int stride_w, int stride_h);
-void splitk_reduce(const at::Tensor& ws, int splits, float* out, long ldo, int M, int N, cudaStream_t stream);
+void splitk_reduce(const at::Tensor& ws, int splits, float* out, long ldo, int M, int N, bool accumulate,
+                   cudaStream_t stream);
 
 static int g_conv_im2col = 1;      // TMA im2col-mode operand fetch where the geometry allows it (C_g % 64 == 0)
 
@@ -556,7 +557,7 @@ void conv_wgrad(const at::Tensor& x, const at::Tensor& dy, at::Tensor dw, at::In
       if (bn == 64) launch_conv<64, true, true, EPI_F32, GATHER_B>(tm, p, cg, grid, stream);
       else launch_conv<128, true, true, EPI_F32, GATHER_B>(tm, p, cg, grid, stream);
     }();
-    if (split > 1) splitk_reduce(ws, static_cast<int>(split), dwg, k_real, Cout_g, static_cast<int>(k_real), stream);
+    if (split > 1) splitk_reduce(ws, static_cast<int>(split), dwg, k_real, Cout_g, static_cast<int>(k_real), true, stream);
   }
 }
 

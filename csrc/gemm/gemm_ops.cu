@@ -270,24 +270,27 @@ splitk_finish_kernel(const float* __restrict__ ws, long split_stride, int splits
   }
 }
 
-// out[m, n] += sum_s ws[s][m, n] in split order (ws: `splits` dense [M, N] fp32 partials, split_stride elements apart).
+// out[m, n] (+)= sum_s ws[s][m, n] in split order (ws: `splits` dense [M, N] fp32 partials, split_stride elements apart).
+// accumulate = 0 overwrites out: gemm_f32(accumulate=False) with split_k > 1 used to add onto whatever out held.
 __global__ void __launch_bounds__(256)
-splitk_reduce_kernel(const float* __restrict__ ws, long split_stride, int splits, float* __restrict__ out, long ldo, int M, int N) {
+splitk_reduce_kernel(const float* __restrict__ ws, long split_stride, int splits, float* __restrict__ out, long ldo, int M, int N,
+                     int accumulate) {
   const long total = static_cast<long>(M) * N;
   for (long i = blockIdx.x * static_cast<long>(blockDim.x) + threadIdx.x; i < total;
        i += static_cast<long>(gridDim.x) * blockDim.x) {
     const long m = i / N, n = i - m * N;
     float v = ws[i];
     for (int sp = 1; sp < splits; ++sp) v += ws[sp * split_stride + i];
-    out[m * ldo + n] += v;
+    if (accumulate) out[m * ldo + n] += v;
+    else out[m * ldo + n] = v;
   }
 }
 
-void splitk_reduce(const at::Tensor& ws, int splits, float* out, long ldo, int M, int N, cudaStream_t stream) {
+void splitk_reduce(const at::Tensor& ws, int splits, float* out, long ldo, int M, int N, bool accumulate, cudaStream_t stream) {
   const long total = static_cast<long>(M) * N;
   const int sms = at::cuda::getCurrentDeviceProperties()->multiProcessorCount;
   const int grid = static_cast<int>(std::max<long>(1, std::min<long>((total + 255) / 256, sms * 8L)));
-  splitk_reduce_kernel<<<grid, 256, 0, stream>>>(ws.data_ptr<float>(), total, splits, out, ldo, M, N);
+  splitk_reduce_kernel<<<grid, 256, 0, stream>>>(ws.data_ptr<float>(), total, splits, out, ldo, M, N, accumulate ? 1 : 0);
   C10_CUDA_KERNEL_LAUNCH_CHECK();
 }
 
@@ -353,8 +356,8 @@ at::Tensor gemm_bf16(const at::Tensor& a, bool a_mn, const at::Tensor& b, bool b
   return c;
 }
 
-// out[M,N] fp32 (+)= alpha * Aᵀ-style product; split_k > 1 adds the product onto out (which must be pre-zeroed or hold the
-// value to accumulate onto): the splits' partials go to a workspace and are summed in split order.
+// out[M,N] fp32 = alpha * A·Bᵀ, or out += alpha * A·Bᵀ with accumulate, for every split_k.  split_k > 1: the splits' partials
+// go to a workspace and are summed in split order, then stored into (or added onto) out in one pass.
 void gemm_f32(const at::Tensor& a, bool a_mn, const at::Tensor& b, bool b_mn, at::Tensor out, double alpha,
               bool accumulate, int64_t split_k, int64_t bn) {
   TORCH_CHECK(a.is_cuda() && a.scalar_type() == at::kBFloat16 && b.scalar_type() == at::kBFloat16);
@@ -386,7 +389,7 @@ void gemm_f32(const at::Tensor& a, bool a_mn, const at::Tensor& b, bool b_mn, at
               {reinterpret_cast<int64_t>(b.data_ptr())}, b_mn, b.stride(0), M, N, K, EPI_F32, p, static_cast<int>(bn), 0,
               stream);
   splitk_reduce(ws, static_cast<int>(splits), out.data_ptr<float>(), out.stride(0), static_cast<int>(M), static_cast<int>(N),
-                stream);
+                accumulate, stream);
 }
 
 // The sufficient-factor outer product with the optimizer fused into the epilogue:
