@@ -14,18 +14,15 @@
 #include <array>
 #include <map>
 #include <mutex>
+#include <vector>
 
 #include "../ops/nhwc_common.cuh"
 #include "wgmma_gemm.cuh"
 
 namespace psd {
 
-void encode_tmap_bf16_2d(CUtensorMap* map, const void* base, int64_t inner, int64_t outer, int64_t ld, int box_inner,
-                         int box_outer);
 void encode_tmap_bf16_3d(CUtensorMap* map, const void* base, int64_t d0, int64_t d1, int64_t d2, int64_t stride1, int64_t stride2,
                          int box0, int box1, int box2);
-void encode_tmap_im2col_bf16(CUtensorMap* map, const void* base, int64_t C, int64_t W, int64_t H, int64_t N, int64_t pitch,
-                             int lower_w, int lower_h, int upper_w, int upper_h, int pixels, int stride_w, int stride_h);
 void splitk_reduce(const at::Tensor& ws, int splits, float* out, long ldo, int M, int N, bool accumulate,
                    cudaStream_t stream);
 
@@ -37,9 +34,12 @@ int pair_cta_enabled();
 extern int g_max_stages;
 extern int g_no_bulk_epi;
 
-template <int BN, bool A_MN, bool B_MN, int EPI, int GATHER, int CG = 1>
+template <int BN, bool A_MN, bool B_MN, int EPI, int GATHER, int CG = 1, typename T = __nv_bfloat16>
 static void launch_conv(const TmapSet& tm, const GemmParams& p, const ConvGeom& cg, int grid, cudaStream_t stream) {
-  auto kern = wgmma_gemm_kernel<BN, A_MN, B_MN, EPI, GATHER, CG>;
+  auto kern = [] {
+    if constexpr (sizeof(T) == 1) return wgmma_fp8_conv_kernel<BN, CG>;
+    else return wgmma_gemm_kernel<BN, A_MN, B_MN, EPI, GATHER, CG>;
+  }();
   constexpr int smem = GemmSmem<BN, CG>::kTotal;
   static bool configured = false;
   if (!configured) {
@@ -205,22 +205,24 @@ static ConvGeom make_geom(const at::Tensor& x, const NhwcView& xv, int c_off, in
   return g;
 }
 
-// TMA im2col eligibility: TAP mode, 64-channel K slices never straddle a tap, corner offsets fit the descriptor.
-// On success fills `map` for boxes of `pixels` base pixels x 64 channels over the gathered tensor.
-static bool im2col_ok(const ConvGeom& g) {
-  if (!g_conv_im2col || g.mode != 0 || g.Cgk % 64 != 0) return false;
+// TMA im2col eligibility: TAP mode, K slices of one 128-byte row (64 bf16 / 128 fp8 channels, `es` bytes per element)
+// never straddle a tap, corner offsets fit the descriptor.
+// On success fills `map` for boxes of `pixels` base pixels x 128 bytes of channels over the gathered tensor.
+static bool im2col_ok(const ConvGeom& g, int es = 2) {
+  if (!g_conv_im2col || g.mode != 0 || g.Cgk % (128 / es) != 0) return false;
   const int org_w = g.off_w - (g.dr < 0 ? g.S - 1 : 0), org_h = g.off_h - (g.dr < 0 ? g.R - 1 : 0);
   // the bounding box must enumerate exactly OW x OH base pixels: extent + upper - lower - 1 = (O - 1) * stride
   const int up_w = (g.OW - 1) * g.sw + 1 + org_w - g.W, up_h = (g.OH - 1) * g.sh + 1 + org_h - g.H;
   auto ok = [](int v) { return v >= -128 && v <= 127; };
   if (!ok(org_w) || !ok(org_h) || !ok(up_w) || !ok(up_h) || g.sw > 8 || g.sh > 8) return false;
-  return (reinterpret_cast<uintptr_t>(g.x) & 15) == 0 && (g.pitch * 2) % 16 == 0;
+  return (reinterpret_cast<uintptr_t>(g.x) & 15) == 0 && (g.pitch * es) % 16 == 0;
 }
-static bool try_im2col_map(CUtensorMap* map, const ConvGeom& g, int pixels) {
-  if (!im2col_ok(g)) return false;
+static bool try_im2col_map(CUtensorMap* map, const ConvGeom& g, int pixels, int es = 2) {
+  if (!im2col_ok(g, es)) return false;
   const int org_w = g.off_w - (g.dr < 0 ? g.S - 1 : 0), org_h = g.off_h - (g.dr < 0 ? g.R - 1 : 0);
   const int up_w = (g.OW - 1) * g.sw + 1 + org_w - g.W, up_h = (g.OH - 1) * g.sh + 1 + org_h - g.H;
-  encode_tmap_im2col_bf16(map, g.x, g.Cg, g.W, g.H, g.N, g.pitch, org_w, org_h, up_w, up_h, pixels, g.sw, g.sh);
+  encode_tmap_im2col(map, g.x, g.Cg, g.W, g.H, g.N, g.pitch, org_w, org_h, up_w, up_h, pixels, g.sw, g.sh,
+                     es == 1 ? CU_TENSOR_MAP_DATA_TYPE_UINT8 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16);
   return true;
 }
 
@@ -270,7 +272,7 @@ at::Tensor conv_fprop(const at::Tensor& x, const at::Tensor& wb, const c10::opti
     const int cl = pick_cluster(m_blocks, m_blocks * n_blocks, sms, &grid);
     TmapSet tm;
     const __nv_bfloat16* wptr = reinterpret_cast<const __nv_bfloat16*>(wb.data_ptr()) + static_cast<long>(gidx) * Cout_g * cg.K;
-    encode_tmap_bf16_2d(&tm.b[0], wptr, cg.K, Cout_g, cg.K, BLOCK_K, bn / cl);     // each CTA multicasts 1/cl of the rows
+    encode_tmap_2d(&tm.b[0], wptr, cg.K, Cout_g, cg.K, BLOCK_K, bn / cl);     // each CTA multicasts 1/cl of the rows
     tm.a[0] = tm.b[0];
     GemmParams p{};
     p.max_stages = g_max_stages;
@@ -293,14 +295,14 @@ at::Tensor conv_fprop(const at::Tensor& x, const at::Tensor& wb, const c10::opti
       if (mc > 1) {
         // cluster multicast of the im2col operand: every CTA fetches 128 / mc pixel rows of the shared A tile
         TORCH_CHECK(try_im2col_map(&tm.a[0], cg, BLOCK_M / mc), "im2col map");
-        encode_tmap_bf16_2d(&tm.b[0], wptr, cg.K, Cout_g, cg.K, BLOCK_K, mbn);
+        encode_tmap_2d(&tm.b[0], wptr, cg.K, Cout_g, cg.K, BLOCK_K, mbn);
         p.cluster = mc;
         launch_im2col_a<1>(mbn, tm, p, cg, mgrid, stream);
         continue;
       }
       if (g_conv_pair && pair_cta_enabled() && m_blocks >= 2 && bn >= 64) {
         // CTA pairs: two pixel blocks share every weight tile; each CTA fetches BN/2 weight rows for both
-        encode_tmap_bf16_2d(&tm.b[0], wptr, cg.K, Cout_g, cg.K, BLOCK_K, bn / 2);
+        encode_tmap_2d(&tm.b[0], wptr, cg.K, Cout_g, cg.K, BLOCK_K, bn / 2);
         launch_im2col_a<2>(bn, tm, p, cg, pair_grid(m_blocks, n_blocks, 1, sms), stream);
         continue;
       }
@@ -310,6 +312,108 @@ at::Tensor conv_fprop(const at::Tensor& x, const at::Tensor& wb, const c10::opti
     TORCH_CHECK(cg.Cgk == cg.Cg, "conv_fprop: channel-padded operand needs the TMA im2col path");
     if (bn == 64) launch_conv<64, false, false, EPI_BF16, GATHER_A>(tm, p, cg, grid, stream);
     else launch_conv<128, false, false, EPI_BF16, GATHER_A>(tm, p, cg, grid, stream);
+  }
+  return y;
+}
+
+// y[N, Cout, OH, OW] (NHWC bf16) = act(conv(x8, w8) * s_x * s_w[co] + bias[co]) with e4m3 operands (fp8_quant.cu):
+//   x8 : e4m3 NHWC, pixel pitch a multiple of 16 bytes;  w8 : [Cout, R*S*Cgk] e4m3, Cgk = per-tap slots (multiple of 128,
+//   slots >= Cg zero);  s_x : one float;  s_w : [Cout] floats.  `out` may be a channel slice of a concat slab.
+// TMA im2col path only: single CTAs, or CTA pairs sharing the weight tile (the default for >= 2 pixel blocks).
+at::Tensor conv_fprop_fp8(const at::Tensor& x8, const at::Tensor& w8, const at::Tensor& s_x, const at::Tensor& s_w,
+                          const c10::optional<at::Tensor>& bias, at::IntArrayRef kernel, at::IntArrayRef stride,
+                          at::IntArrayRef pad, int64_t groups, int64_t OH, int64_t OW, bool relu, double slope,
+                          c10::optional<at::Tensor> out) {
+  TORCH_CHECK(x8.is_cuda() && x8.scalar_type() == at::kFloat8_e4m3fn && w8.scalar_type() == at::kFloat8_e4m3fn &&
+              w8.dim() == 2 && w8.is_contiguous(), "conv_fprop_fp8: e4m3 NHWC x8 and contiguous [Cout, K] e4m3 w8 expected");
+  TORCH_CHECK(s_x.scalar_type() == at::kFloat && s_x.numel() == 1 && s_x.is_cuda(), "conv_fprop_fp8: s_x must be one float");
+  TORCH_CHECK(s_w.scalar_type() == at::kFloat && s_w.is_contiguous() && s_w.numel() == w8.size(0) && s_w.is_cuda(),
+              "conv_fprop_fp8: s_w must hold one float per output channel");
+  TORCH_CHECK(!bias.has_value() || (bias->scalar_type() == at::kFloat && bias->is_contiguous() && bias->numel() == w8.size(0)),
+              "conv_fprop_fp8: bias must be fp32 [Cout]");
+  TORCH_CHECK(g_conv_cluster == 1, "conv_fprop_fp8: the gather multicast-cluster schedule (set_conv_cluster) is bf16-only");
+  TORCH_CHECK(g_conv_mcast == 1, "conv_fprop_fp8: the im2col multicast-cluster schedule (set_conv_mcast) is bf16-only");
+  NhwcView xv = nhwc_view(x8);
+  const int R = static_cast<int>(kernel[0]), S = static_cast<int>(kernel[1]);
+  TORCH_CHECK(groups >= 1 && w8.size(0) % groups == 0 && xv.C % groups == 0, "conv_fprop_fp8: channel counts");
+  const int Cout = w8.size(0), Cout_g = Cout / groups, Cg = xv.C / groups;
+  TORCH_CHECK(Cg % 8 == 0 && R >= 1 && S >= 1, "conv_fprop_fp8: channels per group must be a multiple of 8");
+  TORCH_CHECK(w8.size(1) % (R * S) == 0, "conv_fprop_fp8: weight columns must be R*S*Cgk");
+  const int Cgk = static_cast<int>(w8.size(1) / (R * S));
+  TORCH_CHECK(Cgk % 128 == 0 && Cgk >= Cg, "conv_fprop_fp8: per-tap slots Cgk must be a multiple of 128 and >= Cg");
+  TORCH_CHECK(R <= 15 && S <= 15, "conv_fprop_fp8: kernel extents up to 15 are supported");
+  NhwcView yv{};
+  if (out.has_value()) {
+    yv = nhwc_view(*out);
+    TORCH_CHECK(out->scalar_type() == at::kBFloat16 && yv.C == Cout && yv.H == OH && yv.W == OW && yv.N == xv.N,
+                "conv_fprop_fp8: bad output tensor");
+  }
+  // every group's geometry is validated before any device work
+  std::vector<ConvGeom> geoms(groups);
+  for (int gidx = 0; gidx < groups; ++gidx) {
+    ConvGeom& cg = geoms[gidx];
+    cg.x = reinterpret_cast<const __nv_bfloat16*>(reinterpret_cast<const uint8_t*>(x8.data_ptr()) + gidx * Cg);
+    cg.N = xv.N; cg.H = xv.H; cg.W = xv.W;
+    cg.pitch = xv.pitch;
+    cg.Cg = Cg;
+    cg.Cgk = Cgk;
+    cg.OH = static_cast<int>(OH); cg.OW = static_cast<int>(OW);
+    cg.R = R; cg.S = S;
+    cg.sh = static_cast<int>(stride[0]); cg.sw = static_cast<int>(stride[1]);
+    cg.off_h = -static_cast<int>(pad[0]); cg.off_w = -static_cast<int>(pad[1]);
+    cg.dr = 1;
+    cg.mode = 0;
+    cg.K = R * S * Cgk;
+    cg.M = static_cast<long>(xv.N) * OH * OW;
+    TORCH_CHECK(cg.M < (1L << 31), "conv_fprop_fp8: N*OH*OW must fit in 31 bits");
+    TORCH_CHECK(im2col_ok(cg, 1), "conv_fprop_fp8: geometry outside the im2col-TMA limits (stride <= 8, corner offsets in "
+                "[-128, 127], 16-byte aligned group slices and pixels)");
+    cg.div_ow = make_fastdiv(static_cast<uint32_t>(OW));
+    cg.div_ohow = make_fastdiv(static_cast<uint32_t>(OH * OW));
+    cg.div_cg = make_fastdiv(Cgk);
+    cg.div_s = make_fastdiv(S);
+    cg.scale_x = s_x.data_ptr<float>();
+    cg.scale_w = s_w.data_ptr<float>() + gidx * Cout_g;
+  }
+  c10::cuda::CUDAGuard guard(x8.device());
+  at::Tensor y = out.has_value() ? *out : empty_nhwc(xv.N, Cout, OH, OW, x8.options().dtype(at::kBFloat16));
+  if (!out.has_value()) yv = nhwc_view(y);
+  auto stream = at::cuda::getCurrentCUDAStream();
+  const int sms = at::cuda::getCurrentDeviceProperties()->multiProcessorCount;
+  for (int gidx = 0; gidx < groups; ++gidx) {
+    const ConvGeom& cg = geoms[gidx];
+    TmapSet tm;
+    TORCH_CHECK(try_im2col_map(&tm.a[0], cg, BLOCK_M, 1), "conv_fprop_fp8: im2col map");
+    const long m_blocks = (cg.M + BLOCK_M - 1) / BLOCK_M;
+    const int bn = std::min(pick_conv_bn(Cout_g, m_blocks, sms), 128);
+    const long n_blocks = (Cout_g + bn - 1) / bn;
+    const uint8_t* wptr = reinterpret_cast<const uint8_t*>(w8.data_ptr()) + static_cast<long>(gidx) * Cout_g * cg.K;
+    GemmParams p{};
+    p.max_stages = g_max_stages;
+    p.no_bulk_epi = g_no_bulk_epi;
+    p.cluster = 1;
+    p.M = static_cast<int>(cg.M);
+    p.N = Cout_g;
+    p.kb_per_src = cg.K / 128;
+    p.num_src = 1;
+    p.split_k = 1;
+    p.c_bf16 = reinterpret_cast<__nv_bfloat16*>(y.data_ptr()) + gidx * Cout_g;
+    p.ldc = yv.pitch;
+    p.bias = bias.has_value() ? bias->data_ptr<float>() + gidx * Cout_g : nullptr;
+    p.relu = relu;
+    p.relu_slope = static_cast<float>(slope);
+    p.alpha = 1.f;
+    const bool pair = g_conv_pair && pair_cta_enabled() && m_blocks >= 2;
+    encode_tmap_2d(&tm.b[0], wptr, cg.K, Cout_g, cg.K, 128, pair ? bn / 2 : bn, CU_TENSOR_MAP_DATA_TYPE_UINT8);
+    if (pair) {
+      const int grid = pair_grid(m_blocks, n_blocks, 1, sms);
+      if (bn == 64) launch_conv<64, false, false, EPI_BF16, IM2COL_A, 2, __nv_fp8_e4m3>(tm, p, cg, grid, stream);
+      else launch_conv<128, false, false, EPI_BF16, IM2COL_A, 2, __nv_fp8_e4m3>(tm, p, cg, grid, stream);
+    } else {
+      const int grid = static_cast<int>(std::max<long>(1, std::min<long>(m_blocks * n_blocks, sms)));
+      if (bn == 64) launch_conv<64, false, false, EPI_BF16, IM2COL_A, 1, __nv_fp8_e4m3>(tm, p, cg, grid, stream);
+      else launch_conv<128, false, false, EPI_BF16, IM2COL_A, 1, __nv_fp8_e4m3>(tm, p, cg, grid, stream);
+    }
   }
   return y;
 }
@@ -347,7 +451,7 @@ at::Tensor conv_dgrad(const at::Tensor& dy, const at::Tensor& wt, at::IntArrayRe
     const int cl = pick_cluster(m_blocks, m_blocks * n_blocks, sms, &grid);
     TmapSet tm;
     const __nv_bfloat16* wptr = reinterpret_cast<const __nv_bfloat16*>(wt.data_ptr()) + static_cast<long>(gidx) * Cg * cg.K;
-    encode_tmap_bf16_2d(&tm.b[0], wptr, cg.K, Cg, cg.K, BLOCK_K, bn / cl);
+    encode_tmap_2d(&tm.b[0], wptr, cg.K, Cg, cg.K, BLOCK_K, bn / cl);
     tm.a[0] = tm.b[0];
     GemmParams p{};
     p.max_stages = g_max_stages;
@@ -369,13 +473,13 @@ at::Tensor conv_dgrad(const at::Tensor& dy, const at::Tensor& wt, at::IntArrayRe
       const int mc = plan_im2col_mcast(Cg, m_blocks, sms, &mbn, &mgrid);
       if (mc > 1) {
         TORCH_CHECK(try_im2col_map(&tm.a[0], cg, BLOCK_M / mc), "im2col map");
-        encode_tmap_bf16_2d(&tm.b[0], wptr, cg.K, Cg, cg.K, BLOCK_K, mbn);
+        encode_tmap_2d(&tm.b[0], wptr, cg.K, Cg, cg.K, BLOCK_K, mbn);
         p.cluster = mc;
         launch_im2col_a<1>(mbn, tm, p, cg, mgrid, stream);
         continue;
       }
       if (g_conv_pair && pair_cta_enabled() && m_blocks >= 2 && bn >= 64) {
-        encode_tmap_bf16_2d(&tm.b[0], wptr, cg.K, Cg, cg.K, BLOCK_K, bn / 2);
+        encode_tmap_2d(&tm.b[0], wptr, cg.K, Cg, cg.K, BLOCK_K, bn / 2);
         launch_im2col_a<2>(bn, tm, p, cg, pair_grid(m_blocks, n_blocks, 1, sms), stream);
         continue;
       }
@@ -503,7 +607,7 @@ void conv_wgrad(const at::Tensor& x, const at::Tensor& dy, at::Tensor dw, at::In
     int grid = 0;
     const int cl = pick_cluster(n_blocks, tiles * split, sms, &grid);
     p.cluster = cl;
-    encode_tmap_bf16_2d(&tm.a[0], dyp, Cout_g, cg.M, dv.pitch, 64, BLOCK_K / cl);      // each CTA multicasts 1/cl of the k-rows
+    encode_tmap_2d(&tm.a[0], dyp, Cout_g, cg.M, dv.pitch, 64, BLOCK_K / cl);      // each CTA multicasts 1/cl of the k-rows
     tm.b[0] = tm.a[0];
     p.c_f32 = dw.data_ptr<float>() + static_cast<long>(gidx) * Cout_g * k_real;
     p.ldc = k_real;
@@ -642,6 +746,8 @@ TORCH_LIBRARY_FRAGMENT(poseidon, m) {
   m.def("set_conv_pair(int on) -> ()", &psd::set_conv_pair);
   m.def("conv_fprop(Tensor x, Tensor wb, Tensor? bias, int[] kernel, int[] stride, int[] pad, int groups, int mode, "
         "int OH, int OW, bool relu, float slope, Tensor? out) -> Tensor", &psd::conv_fprop);
+  m.def("conv_fprop_fp8(Tensor x8, Tensor w8, Tensor s_x, Tensor s_w, Tensor? bias, int[] kernel, int[] stride, int[] pad, "
+        "int groups, int OH, int OW, bool relu, float slope, Tensor? out) -> Tensor", &psd::conv_fprop_fp8);
   m.def("conv_dgrad(Tensor dy, Tensor wt, int[] kernel, int[] pad, int groups, int H, int W, Tensor? mask, float slope) "
         "-> Tensor", &psd::conv_dgrad);
   m.def("conv_dgrad_w(Tensor dy, Tensor wb, int[] kernel, int[] pad, int groups, int H, int W, Tensor? mask, float slope) "

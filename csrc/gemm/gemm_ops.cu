@@ -25,16 +25,24 @@ static EncodeFn get_encode_fn() {
   return fn;
 }
 
-// 2-D bf16 tensor map: `inner` contiguous elements, `outer` rows `ld` elements apart, 128B swizzle.
-void encode_tmap_bf16_2d(CUtensorMap* map, const void* base, int64_t inner, int64_t outer, int64_t ld,
-                         int box_inner, int box_outer) {
+static int64_t tmap_elem_bytes(CUtensorMapDataType dtype) {
+  TORCH_CHECK(dtype == CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 || dtype == CU_TENSOR_MAP_DATA_TYPE_UINT8,
+              "tensor maps: bf16 or 8-bit elements");
+  return dtype == CU_TENSOR_MAP_DATA_TYPE_UINT8 ? 1 : 2;
+}
+
+// 2-D tensor map: `inner` contiguous elements, `outer` rows `ld` elements apart, 128B swizzle.  dtype: bf16, or UINT8 for
+// e4m3 operands (the TMA only moves bytes).
+void encode_tmap_2d(CUtensorMap* map, const void* base, int64_t inner, int64_t outer, int64_t ld,
+                    int box_inner, int box_outer, CUtensorMapDataType dtype) {
+  const int64_t es = tmap_elem_bytes(dtype);
   TORCH_CHECK((reinterpret_cast<uintptr_t>(base) & 15) == 0, "TMA base must be 16-byte aligned");
-  TORCH_CHECK((ld * 2) % 16 == 0, "TMA row pitch must be a multiple of 16 bytes (ld=", ld, ")");
+  TORCH_CHECK((ld * es) % 16 == 0, "TMA row pitch must be a multiple of 16 bytes (ld=", ld, ")");
   cuuint64_t dims[2] = {static_cast<cuuint64_t>(inner), static_cast<cuuint64_t>(outer)};
-  cuuint64_t strides[1] = {static_cast<cuuint64_t>(ld) * 2};
+  cuuint64_t strides[1] = {static_cast<cuuint64_t>(ld * es)};
   cuuint32_t box[2] = {static_cast<cuuint32_t>(box_inner), static_cast<cuuint32_t>(box_outer)};
   cuuint32_t estr[2] = {1, 1};
-  CUresult r = get_encode_fn()(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(base), dims, strides,
+  CUresult r = get_encode_fn()(map, dtype, 2, const_cast<void*>(base), dims, strides,
                                box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
                                CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   TORCH_CHECK(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled failed: ", static_cast<int>(r), " inner=", inner,
@@ -56,12 +64,14 @@ void encode_tmap_bf16_3d(CUtensorMap* map, const void* base, int64_t d0, int64_t
   TORCH_CHECK(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled (3-D) failed: ", static_cast<int>(r));
 }
 
-// 4-D im2col-mode bf16 tensor map over an NHWC tensor (channels innermost, pixel pitch `pitch` elements).
+// 4-D im2col-mode tensor map over an NHWC tensor (channels innermost, pixel pitch `pitch` elements).
 //   lower / upper : bounding-box corner offsets {w, h} (cuTensorMapEncodeIm2col semantics: base pixels run from
 //                   `lower` to `extent + upper - 1` in steps of the traversal stride)
-//   box           : `pixels` base pixels x 64 channels, 128B swizzle
-void encode_tmap_im2col_bf16(CUtensorMap* map, const void* base, int64_t C, int64_t W, int64_t H, int64_t N, int64_t pitch,
-                             int lower_w, int lower_h, int upper_w, int upper_h, int pixels, int stride_w, int stride_h) {
+//   box           : `pixels` base pixels x 128 bytes of channels (64 bf16 / 128 e4m3 as UINT8), 128B swizzle
+void encode_tmap_im2col(CUtensorMap* map, const void* base, int64_t C, int64_t W, int64_t H, int64_t N, int64_t pitch,
+                        int lower_w, int lower_h, int upper_w, int upper_h, int pixels, int stride_w, int stride_h,
+                        CUtensorMapDataType dtype) {
+  const int64_t es = tmap_elem_bytes(dtype);
   using Im2colFn = CUresult (*)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
                                 const int*, const int*, cuuint32_t, cuuint32_t, const cuuint32_t*, CUtensorMapInterleave,
                                 CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
@@ -74,14 +84,14 @@ void encode_tmap_im2col_bf16(CUtensorMap* map, const void* base, int64_t C, int6
                 "cuTensorMapEncodeIm2col not available from the driver");
     fn = reinterpret_cast<Im2colFn>(ptr);
   }
-  TORCH_CHECK((reinterpret_cast<uintptr_t>(base) & 15) == 0 && (pitch * 2) % 16 == 0, "im2col TMA: 16-byte alignment");
+  TORCH_CHECK((reinterpret_cast<uintptr_t>(base) & 15) == 0 && (pitch * es) % 16 == 0, "im2col TMA: 16-byte alignment");
   cuuint64_t dims[4] = {static_cast<cuuint64_t>(C), static_cast<cuuint64_t>(W), static_cast<cuuint64_t>(H),
                         static_cast<cuuint64_t>(N)};
-  cuuint64_t strides[3] = {static_cast<cuuint64_t>(pitch) * 2, static_cast<cuuint64_t>(pitch) * W * 2,
-                           static_cast<cuuint64_t>(pitch) * W * H * 2};
+  cuuint64_t strides[3] = {static_cast<cuuint64_t>(pitch * es), static_cast<cuuint64_t>(pitch * W * es),
+                           static_cast<cuuint64_t>(pitch * W * H * es)};
   int lower[2] = {lower_w, lower_h}, upper[2] = {upper_w, upper_h};
   cuuint32_t estr[4] = {1, static_cast<cuuint32_t>(stride_w), static_cast<cuuint32_t>(stride_h), 1};
-  CUresult r = fn(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(base), dims, strides, lower, upper, 64,
+  CUresult r = fn(map, dtype, 4, const_cast<void*>(base), dims, strides, lower, upper, static_cast<cuuint32_t>(128 / es),
                   static_cast<cuuint32_t>(pixels), estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
                   CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   TORCH_CHECK(r == CUDA_SUCCESS, "cuTensorMapEncodeIm2col failed: ", static_cast<int>(r), " C=", C, " W=", W, " H=", H,
@@ -183,10 +193,10 @@ void gemm_launch(const std::vector<int64_t>& a_ptrs, bool a_mn, int64_t lda, con
   int cgp = (g_pair_cta && m_blocks >= 2 && (!b_mn || bn >= 128) && (max_ctas <= 0 || max_ctas >= 2)) ? 2 : 1;
   TmapSet tm;
   for (int s = 0; s < nsrc; ++s) {
-    if (!a_mn) encode_tmap_bf16_2d(&tm.a[s], reinterpret_cast<void*>(a_ptrs[s]), K, M, lda, BLOCK_K, BLOCK_M);
-    else       encode_tmap_bf16_2d(&tm.a[s], reinterpret_cast<void*>(a_ptrs[s]), M, K, lda, 64, BLOCK_K);
-    if (!b_mn) encode_tmap_bf16_2d(&tm.b[s], reinterpret_cast<void*>(b_ptrs[s]), K, N, ldb, BLOCK_K, bn / cgp);
-    else       encode_tmap_bf16_2d(&tm.b[s], reinterpret_cast<void*>(b_ptrs[s]), N, K, ldb, 64, BLOCK_K);
+    if (!a_mn) encode_tmap_2d(&tm.a[s], reinterpret_cast<void*>(a_ptrs[s]), K, M, lda, BLOCK_K, BLOCK_M);
+    else       encode_tmap_2d(&tm.a[s], reinterpret_cast<void*>(a_ptrs[s]), M, K, lda, 64, BLOCK_K);
+    if (!b_mn) encode_tmap_2d(&tm.b[s], reinterpret_cast<void*>(b_ptrs[s]), K, N, ldb, BLOCK_K, bn / cgp);
+    else       encode_tmap_2d(&tm.b[s], reinterpret_cast<void*>(b_ptrs[s]), N, K, ldb, 64, BLOCK_K);
   }
   p.M = static_cast<int>(M);
   p.N = static_cast<int>(N);

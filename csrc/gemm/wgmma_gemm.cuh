@@ -22,6 +22,7 @@
 #pragma once
 #include "sm90_prims.cuh"
 #include "conv_gather.cuh"
+#include <cuda_fp8.h>
 
 namespace psd {
 
@@ -42,6 +43,13 @@ enum GatherMode : int { GATHER_NONE = 0, GATHER_A = 1, GATHER_B = 2, IM2COL_A = 
 __host__ __device__ constexpr bool has_gather_warps(int g) { return g == GATHER_A || g == GATHER_B; }
 
 enum EpiMode : int { EPI_BF16 = 0, EPI_F32 = 1, EPI_SGD = 2 };
+
+// Tensor-map encoders (gemm_ops.cu).  dtype: bf16 operands, or CU_TENSOR_MAP_DATA_TYPE_UINT8 for e4m3 ones.
+void encode_tmap_2d(CUtensorMap* map, const void* base, int64_t inner, int64_t outer, int64_t ld, int box_inner,
+                    int box_outer, CUtensorMapDataType dtype = CU_TENSOR_MAP_DATA_TYPE_BFLOAT16);
+void encode_tmap_im2col(CUtensorMap* map, const void* base, int64_t C, int64_t W, int64_t H, int64_t N, int64_t pitch,
+                        int lower_w, int lower_h, int upper_w, int upper_h, int pixels, int stride_w, int stride_h,
+                        CUtensorMapDataType dtype = CU_TENSOR_MAP_DATA_TYPE_BFLOAT16);
 
 struct TmapSet {
   CUtensorMap a[kMaxSrc];
@@ -124,9 +132,10 @@ __device__ __forceinline__ float sgd_apply(float acc, float& w, float& h, const 
 
 // Epilogue of one 16 x 32 accumulator sub-tile of a warp, already transposed into the warp's padded staging tile
 // (`stage[r * 33 + c]`), so that every global access of the warp is row-contiguous (64-128 B segments).
-template <int EPI>
+// DEQ (fp8 operands, EPI_BF16): the accumulator is first scaled by sx * sw[col], before bias and activation.
+template <int EPI, bool DEQ = false>
 __device__ __forceinline__ void epilogue_tile16(const GemmParams& p, float* c_f32, const float* stage, int lane, int row0,
-                                                int col0) {
+                                                int col0, float sx = 0.f, const float* sw = nullptr) {
   constexpr int ROWS = 16;
   const int nrows = min(ROWS, p.M - row0);
   const int ncols = min(32, p.N - col0);
@@ -138,6 +147,11 @@ __device__ __forceinline__ void epilogue_tile16(const GemmParams& p, float* c_f3
     if (p.bias != nullptr) {
       if (c0) b0 = __ldg(p.bias + col0 + cp);
       if (c1) b1 = __ldg(p.bias + col0 + cp + 1);
+    }
+    [[maybe_unused]] float q0 = 0.f, q1 = 0.f;
+    if constexpr (DEQ) {
+      if (c0) q0 = sx * __ldg(sw + col0 + cp);
+      if (c1) q1 = sx * __ldg(sw + col0 + cp + 1);
     }
     const bool pair_ok = c1 && ((p.ldc & 1) == 0) && (((col0 + cp) & 1) == 0);
     // fused ReLU-backward mask: issue all loads of this lane up front (they are independent), then combine
@@ -163,7 +177,14 @@ __device__ __forceinline__ void epilogue_tile16(const GemmParams& p, float* c_f3
     for (int i = 0; i < ROWS / 2; ++i) {
       const int rr = 2 * i + half;
       if (rr >= nrows) continue;
-      float x0 = stage[rr * 33 + cp] + b0, x1 = stage[rr * 33 + cp + 1] + b1;
+      float x0, x1;
+      if constexpr (DEQ) {
+        x0 = stage[rr * 33 + cp] * q0 + b0;
+        x1 = stage[rr * 33 + cp + 1] * q1 + b1;
+      } else {
+        x0 = stage[rr * 33 + cp] + b0;
+        x1 = stage[rr * 33 + cp + 1] + b1;
+      }
       if (p.relu) {
         x0 = x0 > 0.f ? x0 : x0 * p.relu_slope;
         x1 = x1 > 0.f ? x1 : x1 * p.relu_slope;
@@ -270,11 +291,12 @@ __device__ __forceinline__ void tma_2d(uint32_t dst, const CUtensorMap* map, uin
   if constexpr (CG == 2) tma_load_2d_mcast_u32(dst, map, bar, x, y, 0x3);
   else tma_load_2d_u32(dst, map, bar, x, y);
 }
-template <int BN, bool A_MN, bool B_MN, int CG = 1>
+// KB: elements per k block (one 128-byte row: 64 bf16 or 128 fp8).
+template <int BN, bool A_MN, bool B_MN, int CG = 1, int KB = BLOCK_K>
 struct TmaProducer {
   static_assert(CG == 1 || !B_MN || (BN / CG) % 64 == 0, "MN-major B: each CTA's share must be whole 64-column chunks");
   __device__ static void load_a(const TmapSet& tm, int src, int kb, int m_blk, uint32_t sa, uint32_t bar) {
-    const int k0 = kb * BLOCK_K;
+    const int k0 = kb * KB;
     if constexpr (!A_MN) {
       tma_load_2d_u32(sa, &tm.a[src], bar, k0, m_blk * BLOCK_M);
     } else {
@@ -283,7 +305,7 @@ struct TmaProducer {
     }
   }
   __device__ static void load_b(const TmapSet& tm, int src, int kb, int n_blk, int crank, uint32_t sb, uint32_t bar) {
-    const int k0 = kb * BLOCK_K;
+    const int k0 = kb * KB;
     const int n0 = n_blk * BN + crank * (BN / CG);
     const uint32_t dst = sb + crank * (BN / CG) * 128;         // K-major: BN/CG rows of 128 B; MN-major: BN/CG/64 chunks
     if constexpr (!B_MN) {
@@ -354,9 +376,15 @@ __device__ __forceinline__ TileCoord tile_coord_pair(int t, int m_pairs, int n_b
   return tc;
 }
 
-template <int BN, bool A_MN, bool B_MN, int EPI, int GATHER = GATHER_NONE, int CG = 1>
-__global__ void __launch_bounds__(kNumThreads + (has_gather_warps(GATHER) ? kGatherThreads : 0), 1)
-wgmma_gemm_kernel(const __grid_constant__ TmapSet tm, const GemmParams p, const ConvGeom cg) {
+// Body of the GEMM kernels below.  T: operand element, __nv_bfloat16 or __nv_fp8_e4m3.  A k block is one 128-byte
+// swizzled row either way (64 bf16 or 128 e4m3), so the ring, the descriptors and the TMA boxes keep their byte geometry;
+// fp8 issues k32 MMAs (still 4 per k block) and dequantises in the epilogue (scale_x * scale_w[col], ConvGeom).
+template <int BN, bool A_MN, bool B_MN, int EPI, int GATHER, int CG, typename T>
+__device__ __forceinline__ void wgmma_gemm_body(const TmapSet& tm, const GemmParams p, const ConvGeom cg) {
+  constexpr bool kFp8 = sizeof(T) == 1;
+  constexpr int KB = 128 / static_cast<int>(sizeof(T));     // elements per k block
+  static_assert(sizeof(T) == 2 || (GATHER == IM2COL_A && !A_MN && !B_MN && EPI == EPI_BF16 && BN <= 128),
+                "fp8 operands: K-major im2col fprop with the bf16 epilogue only");
   static_assert(CG == 1 || CG == 2, "one CTA or a CTA pair per B tile");
   static_assert(CG == 1 || !has_gather_warps(GATHER), "CTA pairs share a TMA-fetched B tile");
   static_assert(!has_gather_warps(GATHER) || BN <= kGatherMaxBN, "gather kernels: accumulator register budget");
@@ -487,7 +515,7 @@ wgmma_gemm_kernel(const __grid_constant__ TmapSet tm, const GemmParams p, const 
             TmaProducer<BN, A_MN, B_MN, CG>::load_stage(tm, src, kb, m_blk, n_blk, prank, sa32, sb32, fbar);
           } else if constexpr (GATHER == IM2COL_A) {
             // A tile = 128 output pixels x 64 channels of tap (r, s): one im2col-mode TMA instruction
-            const int k0 = g * BLOCK_K;
+            const int k0 = g * KB;
             const int tap = static_cast<int>(fdiv(static_cast<uint32_t>(k0), cg.div_cg));
             const int c0 = k0 - tap * cg.Cgk;
             const int r = static_cast<int>(fdiv(static_cast<uint32_t>(tap), cg.div_s));
@@ -515,7 +543,7 @@ wgmma_gemm_kernel(const __grid_constant__ TmapSet tm, const GemmParams p, const 
                 else tma_load_3d_u32(sb32 + c * 8192, &tm.b[0], fbar, n0 + 64 * c, in_k ? c0 : 0, in_k ? tap : 0);
               }
             } else {
-              TmaProducer<BN, A_MN, B_MN, CG>::load_b(tm, src, kb, n_blk, prank, sb32, fbar);
+              TmaProducer<BN, A_MN, B_MN, CG, KB>::load_b(tm, src, kb, n_blk, prank, sb32, fbar);
             }
           } else if constexpr (GATHER == IM2COL_B) {
             // B tile = BN/64 chunks of [64 reduction pixels][64 channels of one tap]; the pixels advance with g.
@@ -657,7 +685,7 @@ wgmma_gemm_kernel(const __grid_constant__ TmapSet tm, const GemmParams p, const 
     [[maybe_unused]] const bool bulk_f32 = EPI == EPI_F32 && !p.atomic && !(p.no_bulk_epi & 1) && p.col_cgk == 0 && (p.N & 3) == 0 &&
                                            (p.ldc & 3) == 0 &&
                                            (reinterpret_cast<uintptr_t>(p.c_f32) & 15) == 0 && (p.split_stride & 3) == 0;
-    [[maybe_unused]] const bool bulk_bf16 = EPI == EPI_BF16 && !(p.no_bulk_epi & 2) && (p.N & 7) == 0 && (p.ldc & 7) == 0 &&
+    [[maybe_unused]] const bool bulk_bf16 = EPI == EPI_BF16 && !kFp8 && !(p.no_bulk_epi & 2) && (p.N & 7) == 0 && (p.ldc & 7) == 0 &&
                                             (reinterpret_cast<uintptr_t>(p.c_bf16) & 15) == 0 &&
                                             (p.mask == nullptr || (reinterpret_cast<uintptr_t>(p.mask) & 15) == 0);
     int stage = 0;
@@ -684,7 +712,8 @@ wgmma_gemm_kernel(const __grid_constant__ TmapSet tm, const GemmParams p, const 
                                    : make_smem_desc(a_addr + k * (MMA_K * 2), 16, 1024);
           const uint64_t db = B_MN ? make_smem_desc(b_addr + k * (MMA_K * 128), 8192, 1024)
                                    : make_smem_desc(b_addr + k * (MMA_K * 2), 16, 1024);
-          Wgmma<BN, A_MN ? 1 : 0, B_MN ? 1 : 0>::mma(acc, da, db, 1u);
+          if constexpr (kFp8) WgmmaFp8<BN>::mma(acc, da, db, 1u);
+          else Wgmma<BN, A_MN ? 1 : 0, B_MN ? 1 : 0>::mma(acc, da, db, 1u);
         }
         wgmma_commit();
         wgmma_wait<1>();                          // the previous k-block's MMAs have retired: its slot is free
@@ -805,6 +834,8 @@ wgmma_gemm_kernel(const __grid_constant__ TmapSet tm, const GemmParams p, const 
           // per-warp walk: 16 x 32 sub-tiles transposed through the warp's padded staging tile
           float* stage_w = epi_stage + e * (16 * 33);
           const int row0 = m_blk * BLOCK_M + 16 * e;
+          [[maybe_unused]] float sx = 0.f;
+          if constexpr (kFp8) sx = __ldg(cg.scale_x);
           if (row0 < p.M) {                               // warp-uniform
 #pragma unroll
             for (int c = 0; c < BN / 32; ++c) {
@@ -819,7 +850,8 @@ wgmma_gemm_kernel(const __grid_constant__ TmapSet tm, const GemmParams p, const 
                 }
               }
               __syncwarp();
-              epilogue_tile16<EPI>(p, c_f32, stage_w, lane, row0, col0 + 32 * c);
+              if constexpr (kFp8) epilogue_tile16<EPI, true>(p, c_f32, stage_w, lane, row0, col0 + 32 * c, sx, cg.scale_w);
+              else epilogue_tile16<EPI>(p, c_f32, stage_w, lane, row0, col0 + 32 * c);
               __syncwarp();
             }
           }
@@ -831,6 +863,19 @@ wgmma_gemm_kernel(const __grid_constant__ TmapSet tm, const GemmParams p, const 
 
   __syncthreads();
   if (share > 1) cluster_sync_all();   // no CTA leaves while a peer may still arrive on its barriers / multicast into it
+}
+
+template <int BN, bool A_MN, bool B_MN, int EPI, int GATHER = GATHER_NONE, int CG = 1>
+__global__ void __launch_bounds__(kNumThreads + (has_gather_warps(GATHER) ? kGatherThreads : 0), 1)
+wgmma_gemm_kernel(const __grid_constant__ TmapSet tm, const GemmParams p, const ConvGeom cg) {
+  wgmma_gemm_body<BN, A_MN, B_MN, EPI, GATHER, CG, __nv_bfloat16>(tm, p, cg);
+}
+
+// e4m3 operands: the forward convolution with the im2col-TMA activation operand and the bf16 epilogue (conv_fprop_fp8).
+template <int BN, int CG>
+__global__ void __launch_bounds__(kNumThreads, 1)
+wgmma_fp8_conv_kernel(const __grid_constant__ TmapSet tm, const GemmParams p, const ConvGeom cg) {
+  wgmma_gemm_body<BN, false, false, EPI_BF16, IM2COL_A, CG, __nv_fp8_e4m3>(tm, p, cg);
 }
 
 // Persistent kernels on clusters: a grid holding more clusters than the GPU can run at once would leave its last clusters

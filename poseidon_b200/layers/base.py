@@ -37,7 +37,7 @@ class NetContext:
 
     def __init__(self, phase=P.TRAIN, device="cpu", engine="torch", dtype=torch.float32,
                  rank=0, world_size=1, seed=None, data_shape_hint=None, model_dir=None,
-                 channels_last=False):
+                 channels_last=False, fp8=None):
         self.phase = phase
         self.device = torch.device(device)
         self.engine = engine            # "torch" (cpu / vendor libs) | "sm100" (our kernels)
@@ -48,6 +48,7 @@ class NetContext:
         self.data_shape_hint = data_shape_hint
         self.model_dir = model_dir
         self.channels_last = channels_last
+        self.fp8 = fp8                  # sm100 engine: "off" | "fprop" fp8 forward convolutions (None: POSEIDON_FP8)
 
     @property
     def train(self):

@@ -28,13 +28,16 @@ def plan_sm100(net) -> None:
             consumers.setdefault(b, []).append(i)
 
     # engine state (operand layouts) for every learnable layer
+    fp8 = sm100.resolve_fp8(getattr(net.ctx, "fp8", None))
     for i, layer in enumerate(net.layers):
         if layer.type_name == "CONVOLUTION":
             cin = net.blob_shapes[net.bottom_names[i][0]][1]
             try:
-                sm100.conv_state(layer, cin)
+                st = sm100.conv_state(layer, cin, fp8)
             except ValueError as e:
                 raise ValueError(f"layer {net.layer_names[i]}: {e}") from e
+            if fp8 == "fprop" and net.ctx.rank == 0:
+                log.info("sm100 plan: conv %s: %s (%s)", net.layer_names[i], "fp8" if st.fp8 else "bf16", st.fp8_reason)
         elif layer.type_name == "INNER_PRODUCT" and getattr(layer, "_sm100", None) is None:
             layer._sm100 = sm100.IPState(layer, tuple(net.blob_shapes[net.bottom_names[i][0]]))
 

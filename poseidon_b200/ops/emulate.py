@@ -34,6 +34,29 @@ def _storage_order_flat(t: torch.Tensor) -> torch.Tensor:
     return t.permute(dims).reshape(-1)
 
 
+E4M3 = torch.float8_e4m3fn
+E4M3_MAX = 448.0
+
+
+def _nan_free_abs(v: torch.Tensor) -> torch.Tensor:
+    """|v| with NaN as 0: the kernels' amax uses fmaxf, which skips NaN (an Inf still counts)."""
+    a = v.abs()
+    return torch.where(torch.isnan(a), torch.zeros_like(a), a)
+
+
+def e4m3_scale(amax: torch.Tensor) -> torch.Tensor:
+    """Just-in-time fp8 scale s = 448 / amax in fp32, at most FLT_MAX, and 1 where amax == 0."""
+    amax = amax.float()
+    # a true fp32 division, as the kernels do it (torch computes `448 / t` as 448 * reciprocal(t))
+    s = torch.where(amax > 0, torch.div(torch.full_like(amax, E4M3_MAX), amax), torch.ones_like(amax))
+    return torch.clamp(s, max=torch.finfo(torch.float32).max)
+
+
+def e4m3_quant(v: torch.Tensor, s) -> torch.Tensor:
+    """e4m3(v · s) as cvt.rn.satfinite does it: clamp to ±448 first (torch's cast gives NaN above 464), NaN stays NaN."""
+    return torch.clamp(v.float() * s, -E4M3_MAX, E4M3_MAX).to(E4M3)
+
+
 def _act(v: torch.Tensor, relu: bool, slope: float) -> torch.Tensor:
     if not relu:
         return v
@@ -197,6 +220,46 @@ class EmulatedKernels:
             return t.contiguous()
         out.copy_(t)
         return out
+
+    # ------------------------------------------------------------------------------------------ fp8 forward convolution
+    def fp8_quant_act(self, x, s_x_out):
+        """bf16 NHWC (pitch may exceed C) -> e4m3 [N, C, H, W], a channel slice of a channels-last tensor whose pixel
+        pitch is C rounded up to 16; s_x_out <- 1 / s (csrc/ops/fp8_quant.cu fp8_quant_act)."""
+        n, c, h, w = x.shape
+        v = x.float()
+        s = e4m3_scale(_nan_free_abs(v).amax())
+        s_x_out.copy_(torch.div(torch.ones_like(s), s).reshape(s_x_out.shape))
+        full = torch.zeros((n, (c + 15) // 16 * 16, h, w), dtype=E4M3).contiguous(memory_format=CL)
+        full[:, :c].copy_(e4m3_quant(v, s))
+        return full[:, :c]
+
+    def fp8_quant_weight(self, w, cgk, s_w_out):
+        """fp32 master [Cout, Cg, R, S] -> e4m3 [Cout, R*S*cgk] (slots >= Cg zero), s_w_out[co] <- 1 / s_co
+        (csrc/ops/fp8_quant.cu fp8_quant_weight)."""
+        cout, cg, r, s_ = w.shape
+        rows = w.float().permute(0, 2, 3, 1).reshape(cout, r * s_, cg)
+        s = e4m3_scale(_nan_free_abs(rows).reshape(cout, -1).amax(dim=1))
+        s_w_out.copy_(torch.div(torch.ones_like(s), s))
+        out = torch.zeros((cout, r * s_, cgk), dtype=E4M3)
+        out[..., :cg].copy_(e4m3_quant(rows, s.view(cout, 1, 1)))
+        return out.reshape(cout, r * s_ * cgk)
+
+    def conv_fprop_fp8(self, x8, w8, s_x, s_w, bias, kernel, stride, pad, groups, OH, OW, relu, slope, out):
+        """act(conv(x8, w8) · s_x · s_w[co] + bias[co]) -> bf16 NHWC (csrc/gemm/conv_ops.cu conv_fprop_fp8)."""
+        r, s = kernel
+        cout = w8.shape[0]
+        cg = x8.shape[1] // groups
+        w4 = self._w4_tap(w8.float(), cout, r, s, cg, w8.shape[1] // (r * s))
+        y = F.conv2d(x8.float(), w4, None, tuple(stride), tuple(pad), 1, groups)
+        assert tuple(y.shape[2:]) == (OH, OW), (tuple(y.shape), OH, OW)
+        y = y * (s_x.float().reshape(()) * s_w.float()).view(1, -1, 1, 1)
+        if bias is not None:
+            y = y + bias.float().view(1, -1, 1, 1)
+        y = _act(y, relu, slope)
+        if out is not None:
+            out.copy_(y)
+            return out
+        return _nhwc(y.to(BF16))
 
     # ------------------------------------------------------------------------------------------ elementwise
     def relu_fwd(self, x, slope):

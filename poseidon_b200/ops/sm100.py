@@ -110,13 +110,39 @@ def _pad64(c: int) -> int:
     return p if (p - c) * 100 <= 34 * c else c
 
 
+FP8_MODES = ("off", "fprop")
+
+
+def resolve_fp8(mode: Optional[str] = None) -> str:
+    """The engine's fp8 setting: ``mode`` when given, else ``POSEIDON_FP8`` (unset: "off").
+    "fprop": eligible convolutions run their forward pass on e4m3 operands (data / weight gradients stay bf16)."""
+    m = str(mode if mode is not None else os.environ.get("POSEIDON_FP8", "off")).lower()
+    if m not in FP8_MODES:
+        raise ValueError(f"fp8 must be one of {', '.join(FP8_MODES)}, got '{m}'")
+    return m
+
+
+def fp8_for_engine(engine: str, mode: Optional[str] = None) -> str:
+    """The fp8 setting a net built for ``engine`` runs with.  Only the sm100 engine has fp8 kernels: asking another
+    engine for fp8 explicitly is an error, and ``POSEIDON_FP8`` does not apply to it."""
+    if engine == "sm100":
+        return resolve_fp8(mode)
+    if mode is not None and resolve_fp8(mode) != "off":
+        raise ValueError(f"fp8='{mode}' needs the sm100 engine (engine is '{engine}')")
+    return "off"
+
+
+def _round128(c: int) -> int:
+    return (c + 127) // 128 * 128
+
+
 # =====================================================================================================
 # Convolution
 # =====================================================================================================
 class ConvState:
     """Per-layer engine state: operand layouts + bf16 shadows, refreshed lazily by weight version."""
 
-    def __init__(self, layer, cin_logical: int):
+    def __init__(self, layer, cin_logical: int, fp8: Optional[str] = None):
         self.layer = layer
         self.groups = layer.group
         self.R, self.S = layer.kernel
@@ -169,6 +195,14 @@ class ConvState:
         if not self.row_mode and os.environ.get("POSEIDON_PAD_K", "0") == "1":
             self.cgk = _pad64(self.cg)
             self.cok = _pad64(self.Cout // self.groups)
+        # fp8 forward (opt-in): e4m3 operands quantised on every forward from the input and the fp32 master, Cgk8 slots
+        # per tap (Cg rounded up to 128: one 128-byte K block); decided once here
+        self.fp8, self.fp8_reason = False, "fp8 off"
+        if resolve_fp8(fp8) == "fprop":
+            self.fp8, self.fp8_reason = self._fp8_eligible(layer)
+        self.cgk8 = _round128(self.cg) if self.fp8 else 0
+        self.s_x: Optional[torch.Tensor] = None       # fp8 dequantisation scales, written by the quantisers every forward
+        self.s_w: Optional[torch.Tensor] = None
         self.wbp: Optional[torch.Tensor] = None      # channel-padded copy of wb (derived, refreshed when wb changes)
         self.dirty_wbp = True
         self.wb: Optional[torch.Tensor] = None
@@ -204,6 +238,31 @@ class ConvState:
         self.s2d_hw = (hq, wq)
         self.Rq, self.Sq = rq, sq
         self.Kw = rq * sq * 64
+
+    def _fp8_eligible(self, layer):
+        """(fp8?, reason): TAP mode, channel counts in multiples of 8, an im2col-TMA geometry, and Cg rounded up to 128
+        wasting at most a third of the work (the _pad64 threshold)."""
+        if self.row_mode or self.s2d or self.pad8:
+            return False, "first-layer layout (ROW / s2d / 8-channel pad)"
+        if self.Coutp != self.Cout or self.cg % 8:
+            return False, "channel counts are not multiples of 8"
+        if self.groups > 1 and self.cg % 16:
+            return False, "group slices of the e4m3 input are not 16-byte aligned"
+        (sh, sw), (ph, pw) = layer.stride, layer.pad
+        if sh > 8 or sw > 8:
+            return False, "stride > 8"
+        corners = [-ph, -pw]
+        in_hw = getattr(layer, "in_hw", None)
+        if in_hw is not None:
+            h, w = in_hw
+            oh, ow = (h + 2 * ph - self.R) // sh + 1, (w + 2 * pw - self.S) // sw + 1
+            corners += [(oh - 1) * sh + 1 - ph - h, (ow - 1) * sw + 1 - pw - w]
+        if any(not -128 <= v <= 127 for v in corners):
+            return False, "im2col corner offsets do not fit a signed byte"
+        p = _round128(self.cg)
+        if (p - self.cg) * 100 > 34 * self.cg:
+            return False, f"Cg {self.cg} -> {p} slots wastes more than a third"
+        return True, f"Cg {self.cg} -> {p} slots"
 
     # physical [Cout, Kw] fp32 view of the master weight (TAP mode only)
     def w2d(self) -> torch.Tensor:
@@ -287,10 +346,10 @@ class ConvState:
         return dw.view(self.Cout, self.R, self.S, self.cg).permute(0, 3, 1, 2)   # channels-last strided view
 
 
-def conv_state(layer, cin_logical) -> ConvState:
+def conv_state(layer, cin_logical, fp8: Optional[str] = None) -> ConvState:
     st = getattr(layer, "_sm100", None)
     if st is None:
-        st = ConvState(layer, cin_logical)
+        st = ConvState(layer, cin_logical, fp8)
         layer._sm100 = st
     return st
 
@@ -363,8 +422,12 @@ class _ConvFn(torch.autograd.Function):
             out = None
             if slab is not None and st.Coutp == st.Cout:
                 out = slab[0].slab_view(slab[1], xin.shape[0], oh, ow, xin.device)
-            y = k.conv_fprop(xin, st.operand(), bias, [st.R, st.S], list(stride), list(conv_pad), st.groups,
-                             1 if (st.row_mode and not st.pad8) else 0, oh, ow, relu, float(relu_slope or 0.0), out)
+            if st.fp8:
+                y = _fp8_fprop(k, st, weight, xin, bias, list(stride), list(conv_pad), oh, ow, relu,
+                               float(relu_slope or 0.0), out)
+            else:
+                y = k.conv_fprop(xin, st.operand(), bias, [st.R, st.S], list(stride), list(conv_pad), st.groups,
+                                 1 if (st.row_mode and not st.pad8) else 0, oh, ow, relu, float(relu_slope or 0.0), out)
             if st.Coutp != st.Cout:
                 y = y[:, : st.Cout]            # channel slice of the padded tensor (pixel pitch Coutp)
         ctx.layer, ctx.relu_slope, ctx.conv_pad = layer, relu_slope, conv_pad
@@ -476,6 +539,19 @@ class _ConvFn(torch.autograd.Function):
             else:
                 cur.wait_event(done)            # join: dw / db are complete for whoever consumes them on this stream
         return dx, dw, db, None, None
+
+
+def _fp8_fprop(k, st: ConvState, weight, xin, bias, stride, pad, oh, ow, relu, slope, out):
+    """e4m3 forward: quantise the fp32 master and the input, then the fp8 im2col GEMM.  All three launches run on every
+    forward: under a CUDA graph Python does not run at replay, and the optimizer updates the master inside the graph."""
+    w = weight.detach()
+    if st.s_x is None:
+        st.s_x = torch.ones(1, device=w.device, dtype=torch.float32)
+        st.s_w = torch.ones(st.Cout, device=w.device, dtype=torch.float32)
+    w8 = k.fp8_quant_weight(w, st.cgk8, st.s_w)
+    x8 = k.fp8_quant_act(xin, st.s_x)
+    return k.conv_fprop_fp8(x8, w8, st.s_x, st.s_w, None if bias is None else bias.detach(), [st.R, st.S], stride, pad,
+                            st.groups, oh, ow, relu, slope, out)
 
 
 _DGRAD_PACK = os.environ.get("POSEIDON_DGRAD_PACK", "0") == "1"      # A/B switch: always use the packed dgrad operand

@@ -68,6 +68,9 @@ def make_parser():
     ap.add_argument("--synthetic_shape", default="", help="CxHxW of stand-in data when a DB is absent")
     ap.add_argument("--cuda_graph", default="auto", choices=["auto", "0", "1"],
                     help="replay the training step as one CUDA graph (auto: sm100 engine with the fused backend)")
+    ap.add_argument("--fp8", default=None, choices=["off", "fprop"],
+                    help="sm100 engine: run eligible convolution forward passes on fp8 (e4m3) operands "
+                         "(default: POSEIDON_FP8, else off)")
     ap.add_argument("--stats_json", default="")
     ap.add_argument("--log_level", default="INFO")
     for f in _PS_FLAGS:
@@ -143,7 +146,8 @@ def cmd_train(args) -> int:
                         staleness=args.table_staleness, svb=_bool(args.svb), grad_reduce=args.grad_reduce,
                         model_dir=os.path.dirname(os.path.abspath(args.solver)), data_shape_hint=hint,
                         sfb_mode=args.sfb_mode, aggr_fraction=args.aggr_fraction,
-                        wire_dtype=args.wire_dtype or ("bf16" if str(args.row_oplog_type) == "3" else None))
+                        wire_dtype=args.wire_dtype or ("bf16" if str(args.row_oplog_type) == "3" else None),
+                        fp8=args.fp8)
     if args.cuda_graph != "auto":
         solver.use_cuda_graph = args.cuda_graph == "1"
     if rc.is_root:
@@ -173,13 +177,14 @@ def _build_net(args, phase):
     from .. import proto as P
     from ..layers import NetContext
     from ..net.net import Net
+    from ..ops.sm100 import fp8_for_engine
     dev = torch.device(f"cuda:{args.gpu.split(',')[0] or 0}" if (torch.cuda.is_available() and args.gpu != "-1") else "cpu")
     if dev.type == "cuda":
         torch.cuda.set_device(dev)
     engine = _engine(args, dev)
     ctx = NetContext(phase=phase, device=dev, engine=engine,
                      dtype=torch.bfloat16 if engine == "sm100" else torch.float32,
-                     model_dir=os.path.dirname(os.path.abspath(args.model)))
+                     model_dir=os.path.dirname(os.path.abspath(args.model)), fp8=fp8_for_engine(engine, args.fp8))
     if args.synthetic_shape:
         ctx.data_shape_hint = tuple(int(x) for x in args.synthetic_shape.lower().split("x"))
     net = Net(P.read_net(args.model), phase=phase, ctx=ctx)
