@@ -1,5 +1,7 @@
 """Forward time per fp8-eligible convolution: bf16 (conv_fprop) against fp8 (fp8_quant_weight + fp8_quant_act +
-conv_fprop_fp8), each with its relative error against an fp32 reference of the same layer.
+conv_fprop_fp8), each with its relative error against an fp32 reference of the same layer.  Then the data gradient per
+layer eligible under fp8="fprop+dgrad": bf16 (conv_dgrad_w, the kernel the engine runs for these layers) against fp8
+(fp8_quant_weight_dgrad + fp8_quant_grad + conv_dgrad_fp8), without the producer's ReLU mask.
 
     python benchmarks/fp8_conv_bench.py [--iters 50] [--json out.json]
 
@@ -24,8 +26,9 @@ os.environ.setdefault("POSEIDON_SYNTHETIC_DATA", "1")
 NETS = [("alexnet", 256), ("vgg16", 64), ("googlenet", 32)]
 
 
-def eligible_layers():
-    """(net, layer, N, Cin, H, W, Cout, k, stride, pad, groups, cgk8) of every conv the fp8 plan selects."""
+def eligible_layers(mode="fprop"):
+    """(net, layer, N, Cin, H, W, Cout, k, stride, pad, groups, slots) of every conv the fp8 plan selects: for the forward
+    (mode "fprop", slots = Cgk8) or the data gradient (mode "fprop+dgrad", slots = Cok8)."""
     from poseidon_b200 import proto as P
     from poseidon_b200.layers import NetContext
     from poseidon_b200.models import zoo
@@ -35,11 +38,11 @@ def eligible_layers():
     sm100.set_emulation(True)          # plan on the CPU: only the layer geometry is needed here
     try:
         for name, batch in NETS:
-            ctx = NetContext(phase=P.TRAIN, device="cpu", engine="sm100", dtype=torch.bfloat16, fp8="fprop")
+            ctx = NetContext(phase=P.TRAIN, device="cpu", engine="sm100", dtype=torch.bfloat16, fp8=mode)
             net = Net(getattr(zoo, name)(batch=1, test_batch=1), phase=P.TRAIN, ctx=ctx)
             for i, layer in enumerate(net.layers):
                 st = getattr(layer, "_sm100", None)
-                if layer.type_name != "CONVOLUTION" or not st.fp8:
+                if layer.type_name != "CONVOLUTION" or not (st.fp8_dgrad if mode == "fprop+dgrad" else st.fp8):
                     continue
                 _, c, h, w = net.blob_shapes[net.bottom_names[i][0]]
                 key = (batch, c, h, w, layer.num_output, layer.kernel, layer.stride, layer.pad, layer.group)
@@ -47,7 +50,7 @@ def eligible_layers():
                     continue
                 seen.add(key)
                 out.append((name, net.layer_names[i], batch, c, h, w, layer.num_output, layer.kernel[0], layer.stride[0],
-                            layer.pad[0], layer.group, st.cgk8))
+                            layer.pad[0], layer.group, st.cok8 if mode == "fprop+dgrad" else st.cgk8))
     finally:
         sm100.set_emulation(False)
     return out
@@ -132,9 +135,63 @@ def main():
         if sel:
             tb, tf = sum(r["bf16_ms"] for r in sel), sum(r["fp8_total_ms"] for r in sel)
             print(f"{net}: distinct eligible layers {len(sel)}, bf16 {tb:.3f} ms, fp8 {tf:.3f} ms (x{tb / tf:.2f})")
+    drows = dgrad_rows(k, args.iters)
     if args.json:
         with open(args.json, "w") as f:
-            json.dump(dict(card=card, layers=rows), f, indent=1)
+            json.dump(dict(card=card, layers=rows, dgrad=drows), f, indent=1)
+
+
+def dgrad_rows(k, iters):
+    """Data gradient of every layer the fprop+dgrad plan runs in fp8: bf16 conv_dgrad_w against the three fp8 launches."""
+    rows = []
+    print(f"\n{'data gradient':10s} {'layer':26s} {'shape':28s} {'bf16 ms':>8s} {'qw ms':>7s} {'qdy ms':>7s} "
+          f"{'gemm ms':>8s} {'fp8 ms':>8s} {'speedup':>7s} {'err bf16':>9s} {'err fp8':>9s}")
+    g = torch.Generator(device="cuda").manual_seed(1)
+    for net, name, n, c, h, w, cout, ks, s, p, grp, cok8 in eligible_layers("fprop+dgrad"):
+        cg = c // grp
+        oh, ow = h + 2 * p - ks + 1, w + 2 * p - ks + 1
+        dy = (torch.randn(n, cout, oh, ow, device="cuda", generator=g) * 1e-3).to(torch.bfloat16) \
+            .contiguous(memory_format=torch.channels_last)
+        wm = (torch.randn(cout, cg, ks, ks, device="cuda", generator=g) * (2.0 / (cg * ks * ks)) ** 0.5) \
+            .contiguous(memory_format=torch.channels_last)
+        wb = wm.permute(0, 2, 3, 1).reshape(cout, -1).to(torch.bfloat16).contiguous()
+        s_dy, s_wt = torch.empty(1, device="cuda"), torch.empty(c, device="cuda")
+        geo = ([ks, ks], [p, p], grp, h, w)
+
+        def bf16():
+            return k.conv_dgrad_w(dy, wb, *geo, None, 0.0)
+
+        wt8 = k.fp8_quant_weight_dgrad(wm, grp, cok8, s_wt)
+        dy8, _ = k.fp8_quant_grad(dy, s_dy, None, 0.0)
+
+        def fp8():
+            wt8_ = k.fp8_quant_weight_dgrad(wm, grp, cok8, s_wt)
+            dy8_, _ = k.fp8_quant_grad(dy, s_dy, None, 0.0)
+            return k.conv_dgrad_fp8(dy8_, wt8_, s_dy, s_wt, *geo, None, 0.0)
+
+        t_bf = time_ms(bf16, iters)
+        t_qw = time_ms(lambda: k.fp8_quant_weight_dgrad(wm, grp, cok8, s_wt), iters)
+        t_qd = time_ms(lambda: k.fp8_quant_grad(dy, s_dy, None, 0.0), iters)
+        t_g8 = time_ms(lambda: k.conv_dgrad_fp8(dy8, wt8, s_dy, s_wt, *geo, None, 0.0), iters)
+        t_f8 = time_ms(fp8, iters)
+        ref = torch.nn.grad.conv2d_input((n, c, h, w), wm, dy.float(), 1, p, 1, grp)
+        nref = ref.norm().item()
+        e_bf = (bf16().float() - ref).norm().item() / nref
+        e_f8 = (fp8().float() - ref).norm().item() / nref
+        shape = f"{n}x{cout}x{oh}x{ow}->{c} k{ks}g{grp}"
+        print(f"{net:10s} {name:26s} {shape:28s} {t_bf:8.3f} {t_qw:7.3f} {t_qd:7.3f} {t_g8:8.3f} {t_f8:8.3f} "
+              f"{t_bf / t_f8:7.2f} {e_bf:9.2e} {e_f8:9.2e}")
+        rows.append(dict(net=net, layer=name, shape=shape, bf16_ms=t_bf, quant_w_ms=t_qw, quant_dy_ms=t_qd,
+                         gemm_fp8_ms=t_g8, fp8_total_ms=t_f8, rel_err_bf16=e_bf, rel_err_fp8=e_f8))
+        del dy, wm, wb, wt8, dy8
+        torch.cuda.empty_cache()
+    for net, _ in NETS:
+        sel = [r for r in rows if r["net"] == net]
+        if sel:
+            tb, tf = sum(r["bf16_ms"] for r in sel), sum(r["fp8_total_ms"] for r in sel)
+            print(f"{net} data gradient: distinct eligible layers {len(sel)}, bf16 {tb:.3f} ms, fp8 {tf:.3f} ms "
+                  f"(x{tb / tf:.2f})")
+    return rows
 
 
 if __name__ == "__main__":

@@ -58,10 +58,10 @@ struct ConvGeom {
   int K;                    // total reduction length (multiple of 8)
   long M;                   // N*OH*OW
   FastDiv div_ow, div_ohow, div_cg, div_s, div_lp;
-  // fp8 fprop only: dequantisation scales read by the epilogue (device memory, so a captured graph sees each step's
+  // fp8 kernels only: dequantisation scales read by the epilogue (device memory, so a captured graph sees each step's
   // values).  Kept last so that the kernel-parameter offsets of every other field stay those of the bf16 kernels.
-  const float* scale_x;     // one float: the activation scale
-  const float* scale_w;     // per output column of this group
+  const float* scale_x;     // one float: the activation (fprop) / dY (dgrad) scale
+  const float* scale_w;     // per output column of this group (output channel / input channel)
 };
 
 // Builds the row table (one thread per row).

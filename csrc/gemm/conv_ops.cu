@@ -14,6 +14,7 @@
 #include <array>
 #include <map>
 #include <mutex>
+#include <type_traits>
 #include <vector>
 
 #include "../ops/nhwc_common.cuh"
@@ -37,7 +38,8 @@ extern int g_no_bulk_epi;
 template <int BN, bool A_MN, bool B_MN, int EPI, int GATHER, int CG = 1, typename T = __nv_bfloat16>
 static void launch_conv(const TmapSet& tm, const GemmParams& p, const ConvGeom& cg, int grid, cudaStream_t stream) {
   auto kern = [] {
-    if constexpr (sizeof(T) == 1) return wgmma_fp8_conv_kernel<BN, CG>;
+    if constexpr (std::is_same<T, __nv_fp8_e5m2>::value) return wgmma_fp8_dgrad_kernel<BN, CG>;
+    else if constexpr (sizeof(T) == 1) return wgmma_fp8_conv_kernel<BN, CG>;
     else return wgmma_gemm_kernel<BN, A_MN, B_MN, EPI, GATHER, CG>;
   }();
   constexpr int smem = GemmSmem<BN, CG>::kTotal;
@@ -493,6 +495,111 @@ at::Tensor conv_dgrad(const at::Tensor& dy, const at::Tensor& wt, at::IntArrayRe
   return dx;
 }
 
+// dx[N, Cin, H, W] (NHWC bf16, dense) = conv_transpose(dy8, wt8) * s_dy * s_wt[ci] for stride-1 convolutions, with e5m2 dY
+// and e4m3 weights (fp8_quant.cu):
+//   dy8 : e5m2 NHWC [N, Cout, OH, OW], pixel pitch a multiple of 16 bytes;  wt8 : [groups*Cg, R*S*Cok] e4m3 in
+//   conv_pack_dgrad's order (per group: rows = input channel, K = (r, s, co)), Cok a multiple of 128, slots >= Cout_g zero;
+//   s_dy : one float;  s_wt : [Cin] floats.  Optional mask = forward output of the producer layer, laid out like dx
+//   (fused ReLU backward, as in conv_dgrad).  TMA im2col path only: single CTAs, or CTA pairs sharing the weight tile.
+at::Tensor conv_dgrad_fp8(const at::Tensor& dy8, const at::Tensor& wt8, const at::Tensor& s_dy, const at::Tensor& s_wt,
+                          at::IntArrayRef kernel, at::IntArrayRef pad, int64_t groups, int64_t H, int64_t W,
+                          const c10::optional<at::Tensor>& mask, double slope) {
+  TORCH_CHECK(dy8.is_cuda() && dy8.scalar_type() == at::kFloat8_e5m2 && wt8.is_cuda() &&
+              wt8.scalar_type() == at::kFloat8_e4m3fn && wt8.dim() == 2 && wt8.is_contiguous(),
+              "conv_dgrad_fp8: e5m2 NHWC dy8 and contiguous [Cin, K] e4m3 wt8 expected");
+  TORCH_CHECK(s_dy.is_cuda() && s_dy.scalar_type() == at::kFloat && s_dy.numel() == 1, "conv_dgrad_fp8: s_dy must be one float");
+  TORCH_CHECK(s_wt.is_cuda() && s_wt.scalar_type() == at::kFloat && s_wt.is_contiguous() && s_wt.numel() == wt8.size(0),
+              "conv_dgrad_fp8: s_wt must hold one float per input channel");
+  TORCH_CHECK(kernel.size() == 2 && pad.size() == 2, "conv_dgrad_fp8: kernel and pad take two values");
+  TORCH_CHECK(g_conv_cluster == 1, "conv_dgrad_fp8: the gather multicast-cluster schedule (set_conv_cluster) is bf16-only");
+  TORCH_CHECK(g_conv_mcast == 1, "conv_dgrad_fp8: the im2col multicast-cluster schedule (set_conv_mcast) is bf16-only");
+  NhwcView dv = nhwc_view(dy8);
+  const int R = static_cast<int>(kernel[0]), S = static_cast<int>(kernel[1]);
+  const int ph = static_cast<int>(pad[0]), pw = static_cast<int>(pad[1]);
+  TORCH_CHECK(R >= 1 && S >= 1 && R <= 15 && S <= 15, "conv_dgrad_fp8: kernel extents from 1 to 15 are supported");
+  TORCH_CHECK(ph >= 0 && pw >= 0 && H >= 1 && W >= 1, "conv_dgrad_fp8: bad padding or input extent");
+  TORCH_CHECK(dv.H == H + 2 * ph - R + 1 && dv.W == W + 2 * pw - S + 1,
+              "conv_dgrad_fp8: dY extent is not that of a stride-1 convolution over H x W");
+  TORCH_CHECK(groups >= 1 && wt8.size(0) % groups == 0 && dv.C % groups == 0, "conv_dgrad_fp8: channel counts");
+  const int Cin = static_cast<int>(wt8.size(0)), Cg = Cin / static_cast<int>(groups), Cout_g = dv.C / static_cast<int>(groups);
+  TORCH_CHECK(Cg % 8 == 0 && Cout_g % 8 == 0, "conv_dgrad_fp8: channels per group must be multiples of 8");
+  TORCH_CHECK(wt8.size(1) % (R * S) == 0, "conv_dgrad_fp8: weight columns must be R*S*Cok");
+  const int Cok = static_cast<int>(wt8.size(1) / (R * S));
+  TORCH_CHECK(Cok % 128 == 0 && Cok >= Cout_g, "conv_dgrad_fp8: per-tap slots Cok must be a multiple of 128 and >= Cout_g");
+  if (mask.has_value()) {
+    TORCH_CHECK(mask->is_cuda() && mask->scalar_type() == at::kBFloat16, "conv_dgrad_fp8: bf16 mask expected");
+    NhwcView mv = nhwc_view(*mask);
+    TORCH_CHECK(mv.N == dv.N && mv.C == Cin && mv.H == H && mv.W == W && mv.pitch == Cin,
+                "conv_dgrad_fp8: mask must match dx layout");
+  }
+  // every group's geometry is validated before any device work
+  std::vector<ConvGeom> geoms(groups);
+  for (int gidx = 0; gidx < groups; ++gidx) {
+    ConvGeom& cg = geoms[gidx];
+    cg.x = reinterpret_cast<const __nv_bfloat16*>(reinterpret_cast<const uint8_t*>(dy8.data_ptr()) + gidx * Cout_g);
+    cg.N = dv.N; cg.H = dv.H; cg.W = dv.W;
+    cg.pitch = dv.pitch;
+    cg.Cg = Cout_g;
+    cg.Cgk = Cok;
+    cg.OH = static_cast<int>(H); cg.OW = static_cast<int>(W);
+    cg.R = R; cg.S = S;
+    cg.sh = 1; cg.sw = 1;
+    cg.off_h = ph; cg.off_w = pw;
+    cg.dr = -1;                                 // mirrored tap walk: the transposed convolution
+    cg.mode = 0;
+    cg.K = R * S * Cok;
+    cg.M = static_cast<long>(dv.N) * H * W;
+    TORCH_CHECK(cg.M < (1L << 31), "conv_dgrad_fp8: N*H*W must fit in 31 bits");
+    TORCH_CHECK(im2col_ok(cg, 1), "conv_dgrad_fp8: geometry outside the im2col-TMA limits (mirrored corner offsets in "
+                "[-128, 127], 16-byte aligned group slices and pixels)");
+    cg.div_ow = make_fastdiv(static_cast<uint32_t>(W));
+    cg.div_ohow = make_fastdiv(static_cast<uint32_t>(H * W));
+    cg.div_cg = make_fastdiv(Cok);
+    cg.div_s = make_fastdiv(S);
+    cg.scale_x = s_dy.data_ptr<float>();
+    cg.scale_w = s_wt.data_ptr<float>() + gidx * Cg;
+  }
+  c10::cuda::CUDAGuard guard(dy8.device());
+  at::Tensor dx = empty_nhwc(dv.N, Cin, H, W, dy8.options().dtype(at::kBFloat16));
+  auto stream = at::cuda::getCurrentCUDAStream();
+  const int sms = at::cuda::getCurrentDeviceProperties()->multiProcessorCount;
+  for (int gidx = 0; gidx < groups; ++gidx) {
+    const ConvGeom& cg = geoms[gidx];
+    TmapSet tm;
+    TORCH_CHECK(try_im2col_map(&tm.a[0], cg, BLOCK_M, 1), "conv_dgrad_fp8: im2col map");
+    const long m_blocks = (cg.M + BLOCK_M - 1) / BLOCK_M;
+    const int bn = std::min(pick_conv_bn(Cg, m_blocks, sms), 128);
+    const long n_blocks = (Cg + bn - 1) / bn;
+    const uint8_t* wptr = reinterpret_cast<const uint8_t*>(wt8.data_ptr()) + static_cast<long>(gidx) * Cg * cg.K;
+    GemmParams p{};
+    p.max_stages = g_max_stages;
+    p.no_bulk_epi = g_no_bulk_epi;
+    p.cluster = 1;
+    p.M = static_cast<int>(cg.M);
+    p.N = Cg;
+    p.kb_per_src = cg.K / 128;
+    p.num_src = 1;
+    p.split_k = 1;
+    p.c_bf16 = reinterpret_cast<__nv_bfloat16*>(dx.data_ptr()) + gidx * Cg;
+    p.ldc = Cin;
+    p.mask = mask.has_value() ? reinterpret_cast<const __nv_bfloat16*>(mask->data_ptr()) + gidx * Cg : nullptr;
+    p.relu_slope = static_cast<float>(slope);
+    p.alpha = 1.f;
+    const bool pair = g_conv_pair && pair_cta_enabled() && m_blocks >= 2;
+    encode_tmap_2d(&tm.b[0], wptr, cg.K, Cg, cg.K, 128, pair ? bn / 2 : bn, CU_TENSOR_MAP_DATA_TYPE_UINT8);
+    if (pair) {
+      const int grid = pair_grid(m_blocks, n_blocks, 1, sms);
+      if (bn == 64) launch_conv<64, false, false, EPI_BF16, IM2COL_A, 2, __nv_fp8_e5m2>(tm, p, cg, grid, stream);
+      else launch_conv<128, false, false, EPI_BF16, IM2COL_A, 2, __nv_fp8_e5m2>(tm, p, cg, grid, stream);
+    } else {
+      const int grid = static_cast<int>(std::max<long>(1, std::min<long>(m_blocks * n_blocks, sms)));
+      if (bn == 64) launch_conv<64, false, false, EPI_BF16, IM2COL_A, 1, __nv_fp8_e5m2>(tm, p, cg, grid, stream);
+      else launch_conv<128, false, false, EPI_BF16, IM2COL_A, 1, __nv_fp8_e5m2>(tm, p, cg, grid, stream);
+    }
+  }
+  return dx;
+}
+
 // Data gradient of a stride-1 convolution read straight from the FPROP weight operand wb [Cout][R][S][Cg] (bf16): no
 // packed [Cin][R][S][Cout] copy, no pack kernel per step.  K = (tap, co) with Cok = round64(Cout_g) slots per tap; the
 // surplus slots are zero on both sides (im2col channel overrun on dY, row overrun of the 3-D weight map).  Any Cout_g,
@@ -748,6 +855,8 @@ TORCH_LIBRARY_FRAGMENT(poseidon, m) {
         "int OH, int OW, bool relu, float slope, Tensor? out) -> Tensor", &psd::conv_fprop);
   m.def("conv_fprop_fp8(Tensor x8, Tensor w8, Tensor s_x, Tensor s_w, Tensor? bias, int[] kernel, int[] stride, int[] pad, "
         "int groups, int OH, int OW, bool relu, float slope, Tensor? out) -> Tensor", &psd::conv_fprop_fp8);
+  m.def("conv_dgrad_fp8(Tensor dy8, Tensor wt8, Tensor s_dy, Tensor s_wt, int[] kernel, int[] pad, int groups, int H, int W, "
+        "Tensor? mask, float slope) -> Tensor", &psd::conv_dgrad_fp8);
   m.def("conv_dgrad(Tensor dy, Tensor wt, int[] kernel, int[] pad, int groups, int H, int W, Tensor? mask, float slope) "
         "-> Tensor", &psd::conv_dgrad);
   m.def("conv_dgrad_w(Tensor dy, Tensor wb, int[] kernel, int[] pad, int groups, int H, int W, Tensor? mask, float slope) "

@@ -23,6 +23,7 @@
 #include "sm90_prims.cuh"
 #include "conv_gather.cuh"
 #include <cuda_fp8.h>
+#include <type_traits>
 
 namespace psd {
 
@@ -376,15 +377,19 @@ __device__ __forceinline__ TileCoord tile_coord_pair(int t, int m_pairs, int n_b
   return tc;
 }
 
-// Body of the GEMM kernels below.  T: operand element, __nv_bfloat16 or __nv_fp8_e4m3.  A k block is one 128-byte
-// swizzled row either way (64 bf16 or 128 e4m3), so the ring, the descriptors and the TMA boxes keep their byte geometry;
-// fp8 issues k32 MMAs (still 4 per k block) and dequantises in the epilogue (scale_x * scale_w[col], ConvGeom).
-template <int BN, bool A_MN, bool B_MN, int EPI, int GATHER, int CG, typename T>
+// Body of the GEMM kernels below.  TA / TB: operand elements, both __nv_bfloat16, or fp8 (A __nv_fp8_e4m3 or
+// __nv_fp8_e5m2, B __nv_fp8_e4m3).  A k block is one 128-byte swizzled row either way (64 bf16 or 128 fp8), so the ring,
+// the descriptors and the TMA boxes keep their byte geometry; fp8 issues k32 MMAs (still 4 per k block) and dequantises
+// in the epilogue (scale_x * scale_w[col], ConvGeom).
+template <int BN, bool A_MN, bool B_MN, int EPI, int GATHER, int CG, typename TA, typename TB>
 __device__ __forceinline__ void wgmma_gemm_body(const TmapSet& tm, const GemmParams p, const ConvGeom cg) {
-  constexpr bool kFp8 = sizeof(T) == 1;
-  constexpr int KB = 128 / static_cast<int>(sizeof(T));     // elements per k block
-  static_assert(sizeof(T) == 2 || (GATHER == IM2COL_A && !A_MN && !B_MN && EPI == EPI_BF16 && BN <= 128),
-                "fp8 operands: K-major im2col fprop with the bf16 epilogue only");
+  constexpr bool kFp8 = sizeof(TA) == 1;
+  constexpr bool kE5M2A = std::is_same<TA, __nv_fp8_e5m2>::value;
+  constexpr int KB = 128 / static_cast<int>(sizeof(TA));    // elements per k block
+  static_assert(sizeof(TA) == sizeof(TB), "both operands bf16, or both fp8");
+  static_assert(!kFp8 || std::is_same<TB, __nv_fp8_e4m3>::value, "fp8 B operand: e4m3");
+  static_assert(!kFp8 || (GATHER == IM2COL_A && !A_MN && !B_MN && EPI == EPI_BF16 && BN <= 128),
+                "fp8 operands: K-major im2col convolution with the bf16 epilogue only");
   static_assert(CG == 1 || CG == 2, "one CTA or a CTA pair per B tile");
   static_assert(CG == 1 || !has_gather_warps(GATHER), "CTA pairs share a TMA-fetched B tile");
   static_assert(!has_gather_warps(GATHER) || BN <= kGatherMaxBN, "gather kernels: accumulator register budget");
@@ -712,7 +717,8 @@ __device__ __forceinline__ void wgmma_gemm_body(const TmapSet& tm, const GemmPar
                                    : make_smem_desc(a_addr + k * (MMA_K * 2), 16, 1024);
           const uint64_t db = B_MN ? make_smem_desc(b_addr + k * (MMA_K * 128), 8192, 1024)
                                    : make_smem_desc(b_addr + k * (MMA_K * 2), 16, 1024);
-          if constexpr (kFp8) WgmmaFp8<BN>::mma(acc, da, db, 1u);
+          if constexpr (kE5M2A) WgmmaFp8E5M2<BN>::mma(acc, da, db, 1u);
+          else if constexpr (kFp8) WgmmaFp8<BN>::mma(acc, da, db, 1u);
           else Wgmma<BN, A_MN ? 1 : 0, B_MN ? 1 : 0>::mma(acc, da, db, 1u);
         }
         wgmma_commit();
@@ -868,14 +874,22 @@ __device__ __forceinline__ void wgmma_gemm_body(const TmapSet& tm, const GemmPar
 template <int BN, bool A_MN, bool B_MN, int EPI, int GATHER = GATHER_NONE, int CG = 1>
 __global__ void __launch_bounds__(kNumThreads + (has_gather_warps(GATHER) ? kGatherThreads : 0), 1)
 wgmma_gemm_kernel(const __grid_constant__ TmapSet tm, const GemmParams p, const ConvGeom cg) {
-  wgmma_gemm_body<BN, A_MN, B_MN, EPI, GATHER, CG, __nv_bfloat16>(tm, p, cg);
+  wgmma_gemm_body<BN, A_MN, B_MN, EPI, GATHER, CG, __nv_bfloat16, __nv_bfloat16>(tm, p, cg);
 }
 
 // e4m3 operands: the forward convolution with the im2col-TMA activation operand and the bf16 epilogue (conv_fprop_fp8).
 template <int BN, int CG>
 __global__ void __launch_bounds__(kNumThreads, 1)
 wgmma_fp8_conv_kernel(const __grid_constant__ TmapSet tm, const GemmParams p, const ConvGeom cg) {
-  wgmma_gemm_body<BN, false, false, EPI_BF16, IM2COL_A, CG, __nv_fp8_e4m3>(tm, p, cg);
+  wgmma_gemm_body<BN, false, false, EPI_BF16, IM2COL_A, CG, __nv_fp8_e4m3, __nv_fp8_e4m3>(tm, p, cg);
+}
+
+// e5m2 dY x e4m3 weights: the stride-1 data gradient (conv_dgrad_fp8) — the same im2col-A GEMM with the mirrored tap walk
+// (ConvGeom::dr = -1); the epilogue dequantises per input channel and applies the producer's ReLU mask (p.mask).
+template <int BN, int CG>
+__global__ void __launch_bounds__(kNumThreads, 1)
+wgmma_fp8_dgrad_kernel(const __grid_constant__ TmapSet tm, const GemmParams p, const ConvGeom cg) {
+  wgmma_gemm_body<BN, false, false, EPI_BF16, IM2COL_A, CG, __nv_fp8_e5m2, __nv_fp8_e4m3>(tm, p, cg);
 }
 
 // Persistent kernels on clusters: a grid holding more clusters than the GPU can run at once would leave its last clusters

@@ -38,6 +38,9 @@ def plan_sm100(net) -> None:
                 raise ValueError(f"layer {net.layer_names[i]}: {e}") from e
             if fp8 == "fprop" and net.ctx.rank == 0:
                 log.info("sm100 plan: conv %s: %s (%s)", net.layer_names[i], "fp8" if st.fp8 else "bf16", st.fp8_reason)
+            elif fp8 == "fprop+dgrad" and net.ctx.rank == 0:
+                log.info("sm100 plan: conv %s: %s (%s); dgrad %s (%s)", net.layer_names[i], "fp8" if st.fp8 else "bf16",
+                         st.fp8_reason, "fp8" if st.fp8_dgrad else "bf16", st.fp8_dgrad_reason)
         elif layer.type_name == "INNER_PRODUCT" and getattr(layer, "_sm100", None) is None:
             layer._sm100 = sm100.IPState(layer, tuple(net.blob_shapes[net.bottom_names[i][0]]))
 

@@ -52,6 +52,22 @@ def e4m3_scale(amax: torch.Tensor) -> torch.Tensor:
     return torch.clamp(s, max=torch.finfo(torch.float32).max)
 
 
+E5M2 = torch.float8_e5m2
+E5M2_MAX = 57344.0
+
+
+def e5m2_scale(amax: torch.Tensor) -> torch.Tensor:
+    """Just-in-time e5m2 scale s = 57344 / amax in fp32 (a true division), at most FLT_MAX, and 1 where amax == 0."""
+    amax = amax.float()
+    s = torch.where(amax > 0, torch.div(torch.full_like(amax, E5M2_MAX), amax), torch.ones_like(amax))
+    return torch.clamp(s, max=torch.finfo(torch.float32).max)
+
+
+def e5m2_quant(v: torch.Tensor, s) -> torch.Tensor:
+    """e5m2(v · s) as cvt.rn.satfinite does it: clamp to ±57344 first (torch's cast rounds larger values to inf)."""
+    return torch.clamp(v.float() * s, -E5M2_MAX, E5M2_MAX).to(E5M2)
+
+
 def e4m3_quant(v: torch.Tensor, s) -> torch.Tensor:
     """e4m3(v · s) as cvt.rn.satfinite does it: clamp to ±448 first (torch's cast gives NaN above 464), NaN stays NaN."""
     return torch.clamp(v.float() * s, -E4M3_MAX, E4M3_MAX).to(E4M3)
@@ -260,6 +276,50 @@ class EmulatedKernels:
             out.copy_(y)
             return out
         return _nhwc(y.to(BF16))
+
+    # ------------------------------------------------------------------------------------------ fp8 data gradient
+    def fp8_quant_grad(self, dy, s_out, y, slope):
+        """bf16 NHWC dY (pitch may exceed C) -> (e5m2 [N, C, H, W] as a channel slice of a channels-last tensor whose pixel
+        pitch is C rounded up to 16, the bf16 dY that was cast); s_out <- 1 / s.  With y, dY is first masked as relu_bwd
+        does it (dense result) (csrc/ops/fp8_quant.cu fp8_quant_grad)."""
+        src = dy if y is None else _nhwc(torch.where(y.float() > 0, dy.float(), dy.float() * slope).to(BF16))
+        n, c, h, w = src.shape
+        v = src.float()
+        s = e5m2_scale(_nan_free_abs(v).amax())
+        s_out.copy_(torch.div(torch.ones_like(s), s).reshape(s_out.shape))
+        full = torch.zeros((n, (c + 15) // 16 * 16, h, w), dtype=E5M2).contiguous(memory_format=CL)
+        full[:, :c].copy_(e5m2_quant(v, s))
+        return full[:, :c], src
+
+    def fp8_quant_weight_dgrad(self, w, groups, cok, s_out):
+        """fp32 master [Cout, Cg, R, S] -> e4m3 [groups*Cg, R*S*cok] in conv_pack_dgrad's order (slots >= Cout_g zero),
+        s_out[g*Cg + ci] <- 1 / s per input channel (csrc/ops/fp8_quant.cu fp8_quant_weight_dgrad)."""
+        cout, cg, r, s_ = w.shape
+        cout_g = cout // groups
+        rows = w.float().reshape(groups, cout_g, cg, r * s_).permute(0, 2, 3, 1).reshape(groups * cg, r * s_, cout_g)
+        s = e4m3_scale(_nan_free_abs(rows).reshape(groups * cg, -1).amax(dim=1))
+        s_out.copy_(torch.div(torch.ones_like(s), s))
+        out = torch.zeros((groups * cg, r * s_, cok), dtype=E4M3)
+        out[..., :cout_g].copy_(e4m3_quant(rows, s.view(-1, 1, 1)))
+        return out.reshape(groups * cg, r * s_ * cok)
+
+    def conv_dgrad_fp8(self, dy8, wt8, s_dy, s_wt, kernel, pad, groups, H, W, mask, slope):
+        """Stride-1 data gradient conv_transpose(dy8, wt8) · s_dy · s_wt[ci], producer-ReLU mask in the epilogue
+        (csrc/gemm/conv_ops.cu conv_dgrad_fp8)."""
+        r, s = kernel
+        assert tuple(dy8.shape[2:]) == (H + 2 * pad[0] - r + 1, W + 2 * pad[1] - s + 1), (tuple(dy8.shape), H, W)
+        cout = dy8.shape[1]
+        cout_g = cout // groups
+        cg = wt8.shape[0] // groups
+        cok = wt8.shape[1] // (r * s)
+        w = wt8.float().reshape(groups, cg, r, s, cok)[..., :cout_g]               # g, ci, r, s, co
+        w4 = w.permute(0, 4, 1, 2, 3).reshape(cout, cg, r, s)
+        full = F.conv_transpose2d(dy8.float(), w4, None, 1, 0, 0, groups)
+        dx = full[:, :, pad[0]: pad[0] + H, pad[1]: pad[1] + W]
+        dx = dx * (s_dy.float().reshape(()) * s_wt.float()).view(1, -1, 1, 1)
+        if mask is not None:
+            dx = torch.where(mask.float() > 0, dx, dx * slope)
+        return _nhwc(dx.to(BF16))
 
     # ------------------------------------------------------------------------------------------ elementwise
     def relu_fwd(self, x, slope):

@@ -110,12 +110,14 @@ def _pad64(c: int) -> int:
     return p if (p - c) * 100 <= 34 * c else c
 
 
-FP8_MODES = ("off", "fprop")
+FP8_MODES = ("off", "fprop", "fprop+dgrad")
 
 
 def resolve_fp8(mode: Optional[str] = None) -> str:
     """The engine's fp8 setting: ``mode`` when given, else ``POSEIDON_FP8`` (unset: "off").
-    "fprop": eligible convolutions run their forward pass on e4m3 operands (data / weight gradients stay bf16)."""
+    "fprop": eligible convolutions run their forward pass on e4m3 operands (data / weight gradients stay bf16).
+    "fprop+dgrad": as "fprop", and eligible stride-1 convolutions also compute their data gradient from e5m2 dY and e4m3
+    weights (weight / bias gradients stay bf16 / fp32)."""
     m = str(mode if mode is not None else os.environ.get("POSEIDON_FP8", "off")).lower()
     if m not in FP8_MODES:
         raise ValueError(f"fp8 must be one of {', '.join(FP8_MODES)}, got '{m}'")
@@ -197,12 +199,21 @@ class ConvState:
             self.cok = _pad64(self.Cout // self.groups)
         # fp8 forward (opt-in): e4m3 operands quantised on every forward from the input and the fp32 master, Cgk8 slots
         # per tap (Cg rounded up to 128: one 128-byte K block); decided once here
+        mode = resolve_fp8(fp8)
         self.fp8, self.fp8_reason = False, "fp8 off"
-        if resolve_fp8(fp8) == "fprop":
+        if mode in ("fprop", "fprop+dgrad"):
             self.fp8, self.fp8_reason = self._fp8_eligible(layer)
         self.cgk8 = _round128(self.cg) if self.fp8 else 0
         self.s_x: Optional[torch.Tensor] = None       # fp8 dequantisation scales, written by the quantisers every forward
         self.s_w: Optional[torch.Tensor] = None
+        # fp8 data gradient (opt-in, decided independently of the forward): e5m2 dY x e4m3 weights quantised on every
+        # backward from dY and the fp32 master, Cok8 slots per tap (Cout_g rounded up to 128)
+        self.fp8_dgrad, self.fp8_dgrad_reason = False, "fp8 dgrad off"
+        if mode == "fprop+dgrad":
+            self.fp8_dgrad, self.fp8_dgrad_reason = self._fp8_dgrad_eligible(layer)
+        self.cok8 = _round128(self.Cout // self.groups) if self.fp8_dgrad else 0
+        self.s_dy: Optional[torch.Tensor] = None      # written by the quantisers every backward
+        self.s_wt: Optional[torch.Tensor] = None
         self.wbp: Optional[torch.Tensor] = None      # channel-padded copy of wb (derived, refreshed when wb changes)
         self.dirty_wbp = True
         self.wb: Optional[torch.Tensor] = None
@@ -263,6 +274,31 @@ class ConvState:
         if (p - self.cg) * 100 > 34 * self.cg:
             return False, f"Cg {self.cg} -> {p} slots wastes more than a third"
         return True, f"Cg {self.cg} -> {p} slots"
+
+    def _fp8_dgrad_eligible(self, layer):
+        """(fp8 data gradient?, reason): a stride-1 TAP-mode layer with channel counts in multiples of 8 (Cout_g in
+        multiples of 16 when grouped: the e5m2 group slices of dY start on 16-byte boundaries), mirrored im2col corner
+        offsets in a signed byte, and Cout_g rounded up to 128 wasting at most a third of the work.  The producer mask a
+        fused ReLU hands to this layer is the producer's dense output, laid out like dX (as conv_dgrad requires)."""
+        if self.row_mode or self.s2d or self.pad8:
+            return False, "first-layer layout (ROW / s2d / 8-channel pad)"
+        if tuple(layer.stride) != (1, 1):
+            return False, "strided (bf16 phase decomposition)"
+        cout_g = self.Cout // self.groups
+        if self.Coutp != self.Cout or self.cg % 8 or cout_g % 8:
+            return False, "channel counts are not multiples of 8"
+        if self.groups > 1 and cout_g % 16:
+            return False, "group slices of the e5m2 dY are not 16-byte aligned"
+        if self.R > 15 or self.S > 15:
+            return False, "kernel larger than 15"
+        (ph, pw) = layer.pad
+        # mirrored walk: the box starts at pad - (R - 1) and ends at -pad relative to dY's extent
+        if any(not -128 <= v <= 127 for v in (ph - (self.R - 1), pw - (self.S - 1), -ph, -pw)):
+            return False, "im2col corner offsets do not fit a signed byte"
+        p = _round128(cout_g)
+        if (p - cout_g) * 100 > 34 * cout_g:
+            return False, f"Cout_g {cout_g} -> {p} slots wastes more than a third"
+        return True, f"Cout_g {cout_g} -> {p} slots"
 
     # physical [Cout, Kw] fp32 view of the master weight (TAP mode only)
     def w2d(self) -> torch.Tensor:
@@ -451,7 +487,11 @@ class _ConvFn(torch.autograd.Function):
             dy = dyp
         else:
             dy = as_kernel_input(dy)
-            if y is not None and not st.consumer_masks:
+            if st.fp8_dgrad and ctx.needs_input_grad[0]:
+                # e5m2 dY: amax pass (with this layer's ReLU backward fused in when it masks its own gradient; the
+                # weight / bias gradients below then read the masked bf16 dY it writes) and cast
+                dy8, dy = _fp8_quant_grad(k, st, dy, y if not st.consumer_masks else None, ctx.relu_slope)
+            elif y is not None and not st.consumer_masks:
                 if y.is_contiguous(memory_format=CL) and dy.is_contiguous(memory_format=CL):
                     dy = k.relu_bwd(y, dy, float(ctx.relu_slope))
                 else:                       # y and / or dy are channel slices of a concat slab: pitch-aware kernel
@@ -523,7 +563,12 @@ class _ConvFn(torch.autograd.Function):
                 dx = _strided_dgrad(k, st, layer, dy, xin)
             else:
                 mask = xin if st.mask_input else None
-                if _dgrad_reads_fprop_weights(st, layer, dy):
+                if st.fp8_dgrad:
+                    # e4m3 weights from the fp32 master, then the fp8 im2col GEMM (mirrored taps), on this stream
+                    wt8 = k.fp8_quant_weight_dgrad(layer.weight.detach(), st.groups, st.cok8, st.s_wt)
+                    dx = k.conv_dgrad_fp8(dy8, wt8, st.s_dy, st.s_wt, [st.R, st.S], list(layer.pad), st.groups,
+                                          xin.shape[2], xin.shape[3], mask, 0.0)
+                elif _dgrad_reads_fprop_weights(st, layer, dy):
                     # no packed [Cin][R][S][Cout] copy and no pack kernel per step: the kernel reads the fprop shadow
                     # through a 3-D tensor map as an MN-major B operand
                     dx = k.conv_dgrad_w(dy, st.shadow(), [st.R, st.S], list(layer.pad), st.groups, xin.shape[2],
@@ -552,6 +597,16 @@ def _fp8_fprop(k, st: ConvState, weight, xin, bias, stride, pad, oh, ow, relu, s
     x8 = k.fp8_quant_act(xin, st.s_x)
     return k.conv_fprop_fp8(x8, w8, st.s_x, st.s_w, None if bias is None else bias.detach(), [st.R, st.S], stride, pad,
                             st.groups, oh, ow, relu, slope, out)
+
+
+def _fp8_quant_grad(k, st: ConvState, dy, y, slope):
+    """e5m2 dY for the fp8 data gradient: returns (dy8, the bf16 dY the weight / bias gradients read).  With y (the layer
+    masks its own gradient) the amax pass applies the ReLU backward and writes the masked dY, bit-identical to relu_bwd.
+    Runs on every backward (graph replays included); the scale tensors are allocated once per layer."""
+    if st.s_dy is None:
+        st.s_dy = torch.ones(1, device=dy.device, dtype=torch.float32)
+        st.s_wt = torch.ones(st.Cp, device=dy.device, dtype=torch.float32)
+    return k.fp8_quant_grad(dy, st.s_dy, y, float(slope or 0.0))
 
 
 _DGRAD_PACK = os.environ.get("POSEIDON_DGRAD_PACK", "0") == "1"      # A/B switch: always use the packed dgrad operand

@@ -68,9 +68,9 @@ def make_parser():
     ap.add_argument("--synthetic_shape", default="", help="CxHxW of stand-in data when a DB is absent")
     ap.add_argument("--cuda_graph", default="auto", choices=["auto", "0", "1"],
                     help="replay the training step as one CUDA graph (auto: sm100 engine with the fused backend)")
-    ap.add_argument("--fp8", default=None, choices=["off", "fprop"],
-                    help="sm100 engine: run eligible convolution forward passes on fp8 (e4m3) operands "
-                         "(default: POSEIDON_FP8, else off)")
+    ap.add_argument("--fp8", default=None, choices=["off", "fprop", "fprop+dgrad"],
+                    help="sm100 engine: run eligible convolution forward passes on fp8 (e4m3) operands; fprop+dgrad: "
+                         "also eligible stride-1 data gradients (e5m2 dY x e4m3 weights) (default: POSEIDON_FP8, else off)")
     ap.add_argument("--stats_json", default="")
     ap.add_argument("--log_level", default="INFO")
     for f in _PS_FLAGS:
