@@ -203,6 +203,9 @@ static ConvGeom make_geom(const at::Tensor& x, const NhwcView& xv, int c_off, in
   } else {
     TORCH_CHECK(Cg % 8 == 0 && xv.pitch % 8 == 0 && c_off % 8 == 0, "TAP-mode conv: channels must be multiples of 8");
   }
+  // the gather producers issue 16-byte cp.async copies from g.x: a view that starts between 16-byte boundaries (a channel
+  // slice at an offset that is not a multiple of 8) must fail here, before any launch, not fault on the device
+  TORCH_CHECK((reinterpret_cast<uintptr_t>(g.x) & 15) == 0, "conv: the gathered tensor must start on a 16-byte boundary");
   attach_rowtab(g, x.device().index());
   return g;
 }

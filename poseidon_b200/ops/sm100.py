@@ -87,8 +87,9 @@ def to_nhwc_bf16(x: torch.Tensor) -> torch.Tensor:
 
 
 def _dense_pitch_ok(x: torch.Tensor) -> bool:
-    """NHWC tensor whose only irregularity may be a pixel pitch > C (channel-slice view)."""
-    if x.dim() != 4 or x.stride(1) != 1:
+    """NHWC tensor whose only irregularity may be a pixel pitch > C (channel-slice view), starting on a 16-byte boundary
+    (the kernels read pixels with 16-byte loads: a slice at a channel offset that is not a multiple of 8 is copied)."""
+    if x.dim() != 4 or x.stride(1) != 1 or x.data_ptr() % 16 != 0:
         return False
     n, c, h, w = x.shape
     pitch = x.stride(3) if w > 1 else (x.stride(2) if h > 1 else (x.stride(0) if n > 1 else c))

@@ -180,13 +180,17 @@ def test_gemm_bf16_splitk_finish(k, M, N, ldc, slope, masked):
 
 
 # ------------------------------------------------------------------------------------------------------------ conv_wgrad
-# conv_wgrad schedules (set_conv_mcast, set_conv_pair).  The weight gradient's M dimension is Cout_g: with one m-block
-# (Cout_g <= 128) every schedule launches the single-CTA kernel, so those cases run under the default only.  With two or
-# more m-blocks on the im2col path, "mcast" clusters 2 (3 when the m-blocks divide by 3 and BN >= 192) CTAs along Cout
-# that share the im2col tile by multicast; "pair" takes CTA pairs when the m-block count is even and BN is 128 or 256;
-# "single" is one CTA per tile.
-SCHED = {"mcast": (2, 1), "pair": (1, 1), "single": (1, 0)}
+# conv_wgrad schedules (set_conv_mcast, set_conv_pair, set_conv_im2col, set_conv_cluster).  The weight gradient's M
+# dimension is Cout_g: with one m-block (Cout_g <= 128) every im2col schedule launches the single-CTA kernel, so those cases
+# run under the default only.  With two or more m-blocks on the im2col path, "mcast" clusters 2 (3 when the m-blocks divide
+# by 3 and BN >= 192) CTAs along Cout that share the im2col tile by multicast; "pair" takes CTA pairs when the m-block count
+# is even and BN is 128 or 256; "single" is one CTA per tile.  "gather" builds the im2col operand with the cp.async gather
+# producer instead of TMA; "cluster2" / "cluster4" do so in clusters of 2 / 4 CTAs along the K columns that share the dY
+# tile by multicast.  A channel-padded reduction needs the im2col path, so its cases skip these three.
+SCHED = {"mcast": (2, 1, 1, 1), "pair": (1, 1, 1, 1), "single": (1, 0, 1, 1),          # (mcast, pair, im2col, cluster)
+         "gather": (1, 1, 0, 1), "cluster2": (1, 1, 1, 2), "cluster4": (1, 1, 1, 4)}
 ALL = ("mcast", "pair", "single")
+GATHER = ("gather", "cluster2", "cluster4")
 CONV_W = [
     # (N, Cin, H, W, Cout, k, stride, pad, group, cgk), schedules whose kernels differ
     ((2, 40, 9, 9, 72, 3, 1, 1, 1, 0), ("pair",)),        # gather (C_g 40), N·OH·OW = 162: one split, one atomic add each
@@ -197,27 +201,35 @@ CONV_W = [
     ((4, 64, 28, 28, 128, 3, 1, 1, 1, 0), ("pair",)),     # im2col, 3136 pixels: per-split workspace + ordered reduce
     ((4, 96, 27, 27, 256, 5, 1, 2, 2, 0), ("pair",)),     # grouped gather (C_g 48), 2916 pixels: workspace
     ((2, 96, 28, 28, 128, 3, 1, 1, 1, 128), ("pair",)),   # channel-padded reduction, 1568 pixels: workspace
-    ((2, 128, 14, 14, 256, 3, 1, 1, 1, 0), ALL),          # 2 m-blocks, BN 256, one split: cluster of 2 / pair / single
-    ((2, 64, 14, 14, 256, 3, 1, 1, 1, 0), ("mcast", "single")),   # 2 m-blocks, BN 192 (no pairs), one split
-    ((2, 64, 14, 14, 384, 3, 1, 1, 1, 0), ("mcast", "single")),   # 3 m-blocks, BN 192: cluster of 3, one split
-    ((4, 128, 28, 28, 256, 3, 1, 1, 1, 0), ALL),          # 2 m-blocks, 3136 pixels: workspace under every schedule
-    ((2, 256, 28, 28, 512, 3, 1, 1, 2, 0), ALL),          # grouped, Cout_g 256, 1568 pixels: workspace per group
+    ((2, 128, 14, 14, 256, 3, 1, 1, 1, 0), ALL + GATHER), # 2 m-blocks, BN 256, one split: cluster of 2 / pair / single
+    ((2, 64, 14, 14, 256, 3, 1, 1, 1, 0), ("mcast", "single") + GATHER),   # 2 m-blocks, BN 192 (no pairs), one split
+    ((2, 64, 14, 14, 384, 3, 1, 1, 1, 0), ("mcast", "single") + GATHER),   # 3 m-blocks, BN 192: cluster of 3, one split
+    ((4, 128, 28, 28, 256, 3, 1, 1, 1, 0), ALL + GATHER), # 2 m-blocks, 3136 pixels: workspace under every schedule
+    ((2, 256, 28, 28, 512, 3, 1, 1, 2, 0), ALL + GATHER), # grouped, Cout_g 256, 1568 pixels: workspace per group
     ((2, 96, 28, 28, 256, 3, 1, 1, 1, 128), ALL),         # channel-padded, 2 m-blocks, workspace
+    # rectangular 3x5, stride (2,1), pad (1,2): 2 m-blocks, on the im2col and the gather paths
+    ((2, 64, 13, 21, 192, (3, 5), (2, 1), (1, 2), 1, 0), ("pair", "single") + GATHER),
 ]
 CONV_W_PARAMS = [pytest.param(c, sc, id="x".join(map(str, c)) + "-" + sc) for c, scheds in CONV_W for sc in scheds]
+
+
+def _hw(v):
+    """(h, w) of a kernel / stride / pad given as one int or a pair."""
+    return tuple(v) if isinstance(v, tuple) else (v, v)
 
 
 @functools.lru_cache(maxsize=None)
 def _conv_case(case):
     n, cin, h, w, cout, kk, stride, pad, group, cgk = case
+    (r, s), (sh, sw), (ph, pw) = _hw(kk), _hw(stride), _hw(pad)
     cg = cin // group
     x = _randn((n, cin, h, w), 11, dtype=BF16).contiguous(memory_format=CL)
-    oh, ow = (h + 2 * pad - kk) // stride + 1, (w + 2 * pad - kk) // stride + 1
+    oh, ow = (h + 2 * ph - r) // sh + 1, (w + 2 * pw - s) // sw + 1
     dy = _randn((n, cout, oh, ow), 12, dtype=BF16).contiguous(memory_format=CL)
 
     def wg(a, b):
-        g = torch.nn.grad.conv2d_weight(a, (cout, cg, kk, kk), b, stride, pad, 1, group)
-        return g.permute(0, 2, 3, 1).reshape(cout, kk * kk * cg)
+        g = torch.nn.grad.conv2d_weight(a, (cout, cg, r, s), b, (sh, sw), (ph, pw), 1, group)
+        return g.permute(0, 2, 3, 1).reshape(cout, r * s * cg)
     ref = wg(x.double(), dy.double())
     mag = wg(x.double().abs(), dy.double().abs())
     return x, dy, ref, mag, n * oh * ow
@@ -228,21 +240,26 @@ def _conv_case(case):
 def test_conv_wgrad_accumulates(k, case, sched, alpha):
     """conv_wgrad adds alpha·dW onto a pre-filled, guard-banded gradient sink (a layer sharing its weight with another
     relies on that) — through one split's atomics and through the workspace + ordered reduce, under the single-CTA,
-    CTA-pair and multicast-cluster schedules."""
+    CTA-pair, multicast-cluster, gather and gather-cluster schedules."""
     dev = _dev(k)
-    mc, pair = SCHED[sched]
+    mc, pair, im2col, cluster = SCHED[sched]
     n, cin, h, w, cout, kk, stride, pad, group, cgk = case
     x, dy, ref, mag, red = _conv_case(case)
-    kw = kk * kk * (cin // group)
+    kernel = _hw(kk)
+    kw = kernel[0] * kernel[1] * (cin // group)
     dw0 = _randn((cout, kw), 13, 10.0)
     buf, dw = _guarded((cout, kw), (kw, 1), torch.float32, dev, dw0)
     try:
         k.set_conv_mcast(mc)
         k.set_conv_pair(pair)
-        k.conv_wgrad(x.to(dev), dy.to(dev), dw, [kk, kk], [stride, stride], [pad, pad], group, 0, alpha, cgk)
+        k.set_conv_im2col(im2col)
+        k.set_conv_cluster(cluster)
+        k.conv_wgrad(x.to(dev), dy.to(dev), dw, list(kernel), list(_hw(stride)), list(_hw(pad)), group, 0, alpha, cgk)
     finally:
         k.set_conv_mcast(1)
         k.set_conv_pair(1)
+        k.set_conv_im2col(1)
+        k.set_conv_cluster(1)
     want = dw0.double() + alpha * ref
     bound = C_GEMM * red * U * (abs(alpha) * mag + dw0.double().abs())
     _within(dw, want, bound, "conv_wgrad")

@@ -37,19 +37,22 @@ def test_lrn_fwd_bwd(ext, shape):
 
 @pytest.mark.parametrize("shape,k,s,p", [((4, 96, 55, 55), 3, 2, 0), ((2, 256, 13, 13), 3, 2, 0),
                                           ((2, 64, 28, 28), 3, 1, 1), ((2, 192, 56, 56), 3, 2, 0),
-                                          ((2, 128, 14, 14), 5, 3, 0)])
+                                          ((2, 128, 14, 14), 5, 3, 0),
+                                          ((2, 64, 13, 11), (3, 2), (2, 1), (1, 0)),      # rectangular window / stride / pad
+                                          ((3, 96, 9, 16), (2, 3), (1, 2), (0, 1))])
 @pytest.mark.parametrize("is_max", [True, False])
 def test_pool_fwd_bwd(ext, shape, k, s, p, is_max):
     from poseidon_b200.ops import sm100
+    k, s, p = _pair(k), _pair(s), _pair(p)
     x = _nhwc(shape, 3)
     xr = x.float().contiguous().requires_grad_(True)      # oracle on plain NCHW fp32
     fn_r = R.max_pool if is_max else R.ave_pool
-    yr = fn_r(xr, (k, k), (s, s), (p, p))
+    yr = fn_r(xr, k, s, p)
     dy = _nhwc(tuple(yr.shape), 4)
     yr.backward(dy.float().contiguous())
     xs = x.clone().requires_grad_(True)
     fn = sm100.max_pool if is_max else sm100.ave_pool
-    y = fn(xs, (k, k), (s, s), (p, p))
+    y = fn(xs, k, s, p)
     assert tuple(y.shape) == tuple(yr.shape)
     y.backward(dy)
     _close(y, yr, what="pool fwd")
@@ -126,13 +129,18 @@ def test_transform_kernel_matches_reference(ext):
 
 
 # ---------------------------------------------------------------------------------------------------- conv
+def _pair(v):
+    return tuple(v) if isinstance(v, (tuple, list)) else (v, v)
+
+
 class _FakeLayer:
+    """A conv layer's attributes; kernel, stride and pad take an int or an (h, w) pair."""
     def __init__(self, cout, cin, k, stride, pad, group, bias=True):
         self.layer_name = "conv"
-        self.num_output, self.kernel, self.stride, self.pad, self.group = cout, (k, k), (stride, stride), (pad, pad), group
+        self.num_output, self.kernel, self.stride, self.pad, self.group = cout, _pair(k), _pair(stride), _pair(pad), group
         self.bias_term = bias
-        g = torch.Generator(device="cuda").manual_seed(cout + cin + k)
-        self.weight = torch.nn.Parameter(torch.randn(cout, cin // group, k, k, generator=g, device="cuda") * 0.05)
+        g = torch.Generator(device="cuda").manual_seed(cout + cin + self.kernel[0] + 16 * (self.kernel[1] - self.kernel[0]))
+        self.weight = torch.nn.Parameter(torch.randn(cout, cin // group, *self.kernel, generator=g, device="cuda") * 0.05)
         self.bias = torch.nn.Parameter(torch.randn(cout, generator=g, device="cuda") * 0.1) if bias else None
         self.in_hw = None
 
