@@ -152,6 +152,10 @@ lrn_reg_kernel(const __nv_bfloat16* __restrict__ x, const __nv_bfloat16* __restr
     const int v = static_cast<int>(i - p * div_c8.d);
     float xw[24];                                 // channels [8v-8, 8v+16)
     load_window<0>(x + static_cast<long>(p) * xpitch + v * 8, v, c8, xw);
+    if (mask_relu) {                              // the op is applied to ReLU(x), as in the shared-memory kernel
+#pragma unroll
+      for (int q = 0; q < 24; ++q) xw[q] = fmaxf(xw[q], 0.f);
+    }
     float o[8];
     if constexpr (!BWD) {
       // sliding window over the squares of channels [8v-pre, 8v+7+pre]

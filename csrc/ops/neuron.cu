@@ -47,6 +47,7 @@ __device__ __forceinline__ float unary_bwd(float s, float dy, const UnaryParams&
     return dy * e / (e + 1.f);
   }
   if constexpr (OP == U_POWER) {
+    if (p.a * p.b == 0.f) return dy * 0.f;      // power_layer.cu:42: powf(0, a - 1) would make 0 * inf = NaN
     if (p.a == 1.f) return dy * p.b;
     const float v = p.c + p.b * s;
     if (p.a == 2.f) return dy * 2.f * p.b * v;

@@ -98,7 +98,9 @@ pool_fwd_kernel(const __nv_bfloat16* __restrict__ x, __nv_bfloat16* __restrict__
           for (int j = 0; j < 8; ++j) acc[j] += f[j];
         }
       }
-      const float inv = 1.f / static_cast<float>((he_pad - hs) * (we_pad - ws));
+      // a window that starts at or past H + pad (ceil mode with k < s, pad 0) is empty: 0, not 0 / 0
+      const int pool_size = (he_pad - hs) * (we_pad - ws);
+      const float inv = pool_size > 0 ? 1.f / static_cast<float>(pool_size) : 0.f;
 #pragma unroll
       for (int j = 0; j < 8; ++j) acc[j] *= inv;
       st8(y + static_cast<long>(opix) * g.ypitch + v * 8, pack8(acc));

@@ -383,9 +383,10 @@ class EmulatedKernels:
         return _nhwc(R.lrn_across(xf, size, alpha, beta).to(BF16))
 
     def lrn_bwd(self, x, dy, size, alpha, beta, fuse_relu):
-        """dx of across-channel LRN; fuse_relu zeroes the gradient where the (post-ReLU) input is not positive
-        (csrc/ops/lrn.cu:140-210)."""
-        xf = x.float().detach().requires_grad_(True)
+        """dx of across-channel LRN; with fuse_relu, of LRN(ReLU(x)) and zero where x is not positive
+        (csrc/ops/lrn.cu:140-215)."""
+        xr = x.float().clamp_min(0) if fuse_relu else x.float()
+        xf = xr.detach().requires_grad_(True)
         with torch.enable_grad():
             y = R.lrn_across(xf, size, alpha, beta)
         (dx,) = torch.autograd.grad(y, xf, dy.float())
@@ -393,29 +394,64 @@ class EmulatedKernels:
             dx = dx * (x.float() > 0)
         return _nhwc(dx.to(BF16))
 
+    @staticmethod
+    def _pool_plane(in_hw, out_hw, k, s, p):
+        """Extent of the zero-based plane that holds the image at offset (p_h, p_w) and every window of Caffe's
+        ceil-mode pooling: with k < s and no pad, the last window may start past the image."""
+        return tuple(max((o - 1) * st + kk, p_ + i) for i, o, kk, st, p_ in zip(in_hw, out_hw, k, s, p))
+
+    def _pool_windows(self, x, k, s, p, oh, ow, fill):
+        """(N, C, OH, OW, kh*kw) windows in row-major tap order over the plane, `fill` outside the image; plane extent."""
+        n, c, h, w = x.shape
+        ph_, pw_ = self._pool_plane((h, w), (oh, ow), k, s, p)
+        plane = torch.full((n, c, ph_, pw_), fill, dtype=torch.float32)
+        plane[:, :, p[0]: p[0] + h, p[1]: p[1] + w] = x.float()
+        cols = plane.as_strided((n, c, oh, ow, k[0], k[1]), (c * ph_ * pw_, ph_ * pw_, s[0] * pw_, s[1], pw_, 1))
+        return cols.reshape(n, c, oh, ow, k[0] * k[1]), (ph_, pw_)
+
+    @staticmethod
+    def _ave_inv(in_hw, out_hw, k, s, p):
+        """[OH, OW] 1 / pool_size, pool_size from the window clipped to H + pad (0 for an empty window)."""
+        ext = []
+        for i, o, kk, st, p_ in zip(in_hw, out_hw, k, s, p):
+            start = torch.arange(o) * st - p_
+            ext.append(torch.clamp(start + kk, max=i + p_) - start)
+        size = ext[0].view(-1, 1) * ext[1].view(1, -1)
+        return torch.where(size > 0, 1.0 / size.clamp_min(1).float(), torch.zeros(()))
+
+    @staticmethod
+    def _tap_to_plane(tap, k, s, pw_):
+        oh, ow = tap.shape[2:]
+        rows = torch.arange(oh).view(1, 1, oh, 1) * s[0] + tap // k[1]
+        cols = torch.arange(ow).view(1, 1, 1, ow) * s[1] + tap % k[1]
+        return rows * pw_ + cols
+
     def pool_fwd(self, x, is_max, k, s, p, oh, ow, want_idx):
-        """(y, idx).  The kernel's idx is the in-window tap of the maximum, one byte per output element
-        (csrc/ops/pool.cu:28-110); it is opaque to the caller, so the emulation stores the plane index instead."""
-        xf = x.float()
+        """(y, idx) with Caffe's window rules (csrc/ops/pool.cu:28-110): the window is clipped to the image for MAX and
+        the sum, to H + pad for the AVE divisor; the first maximum in row-major window order wins; an empty window gives
+        -inf (MAX) or 0 (AVE).  The kernel's idx is the in-window tap of the maximum; it is opaque to the caller, so the
+        emulation stores the index into the padded plane of _pool_plane instead."""
+        h, w = x.shape[2:]
+        cols, (_, pw_) = self._pool_windows(x, k, s, p, oh, ow, float("-inf") if is_max else 0.0)
         if is_max:
-            y, idx = F.max_pool2d(xf, tuple(k), tuple(s), tuple(p), ceil_mode=True, return_indices=True)
-            y, idx = y[:, :, :oh, :ow], idx[:, :, :oh, :ow]
-            assert tuple(y.shape[2:]) == (oh, ow)
-            return _nhwc(y.to(BF16)), (idx.contiguous() if want_idx else torch.empty(0, dtype=torch.int64))
-        y = R.ave_pool(xf, tuple(k), tuple(s), tuple(p))[:, :, :oh, :ow]
-        return _nhwc(y.to(BF16)), torch.empty(0, dtype=torch.int64)
+            y, tap = cols.max(-1)
+            return _nhwc(y.to(BF16)), (self._tap_to_plane(tap, k, s, pw_) if want_idx else torch.empty(0, dtype=torch.int64))
+        return _nhwc((cols.sum(-1) * self._ave_inv((h, w), (oh, ow), k, s, p)).to(BF16)), torch.empty(0, dtype=torch.int64)
 
     def pool_bwd(self, dy, idx, is_max, in_hw, k, s, p):
-        n, c = dy.shape[:2]
+        n, c, oh, ow = dy.shape
         h, w = in_hw
+        ph_, pw_ = self._pool_plane((h, w), (oh, ow), k, s, p)
         if is_max:
-            dx = torch.zeros(n, c, h * w, dtype=torch.float32)
-            dx.scatter_add_(2, idx.reshape(n, c, -1), dy.float().reshape(n, c, -1))
-            return _nhwc(dx.view(n, c, h, w).to(BF16))
-        xf = torch.zeros(n, c, h, w, requires_grad=True)
-        with torch.enable_grad():
-            y = R.ave_pool(xf, tuple(k), tuple(s), tuple(p))
-        (dx,) = torch.autograd.grad(y, xf, dy.float())
+            plane = torch.zeros(n, c, ph_ * pw_, dtype=torch.float32)
+            plane.scatter_add_(2, idx.reshape(n, c, -1), dy.float().reshape(n, c, -1))
+        else:
+            g = dy.float() * self._ave_inv((h, w), (oh, ow), k, s, p)
+            plane = torch.zeros(n, c, ph_, pw_, dtype=torch.float32)
+            for i in range(k[0]):
+                for j in range(k[1]):
+                    plane[:, :, i: i + (oh - 1) * s[0] + 1: s[0], j: j + (ow - 1) * s[1] + 1: s[1]] += g
+        dx = plane.view(n, c, ph_, pw_)[:, :, p[0]: p[0] + h, p[1]: p[1] + w]
         return _nhwc(dx.to(BF16))
 
     # ------------------------------------------------------------------------------------------ layer kernels (round 2)
@@ -445,7 +481,10 @@ class EmulatedKernels:
             d = g * e / (e + 1)
         elif op == 4:
             v = c + b * s
-            d = g * b if a == 1 else (g * 2 * b * v if a == 2 else g * a * b * v.pow(a - 1))
+            if a * b == 0:
+                d = g * 0.0                   # power_layer.cu:42 (v.pow(a - 1) can be inf where v == 0)
+            else:
+                d = g * b if a == 1 else (g * 2 * b * v if a == 2 else g * a * b * v.pow(a - 1))
         else:
             d = torch.zeros_like(g)
         return self._like(dy, d)
@@ -526,37 +565,34 @@ class EmulatedKernels:
     def stochastic_pool_fwd(self, x, k, s, oh, ow, train, seed, iter_dev):
         """(y, idx): idx is opaque to the caller (fed back to pool_bwd), so the emulation stores the plane index like
         its pool_fwd does (csrc/ops/lrn_within.cu: the kernel stores the in-window tap)."""
-        xf = x.float()
-        cols, oh2, ow2 = R._pool_windows(xf, tuple(k), tuple(s))
-        assert (oh2, ow2) == (oh, ow)
-        ssum = cols.sum(-1)
+        cols, (_, pw_) = self._pool_windows(x, k, s, (0, 0), oh, ow, 0.0)
+        run = cols.cumsum(-1)
+        ssum = run[..., -1]                   # taps outside the image add 0: a pick never lands on one
         if not train:
-            y = (cols * cols).sum(-1) / ssum.clamp_min(torch.finfo(torch.float32).tiny)
+            y = torch.where(ssum > 0, (cols * cols).sum(-1) / ssum, torch.zeros(()))
             return _nhwc(y.to(BF16)), torch.empty(0, dtype=torch.int64)
         it = int(iter_dev.item()) if iter_dev is not None else 0
         g = torch.Generator().manual_seed((int(seed) ^ (it * 0x9E3779B97F4A7C15)) & 0x7FFFFFFFFFFFFFFF)
         thr = torch.rand(ssum.shape, generator=g) * ssum
-        tap = (cols.cumsum(-1) < thr.unsqueeze(-1)).sum(-1).clamp_max(cols.shape[-1] - 1)
+        tap = (run < thr.unsqueeze(-1)).sum(-1).clamp_max(cols.shape[-1] - 1)
         y = cols.gather(-1, tap.unsqueeze(-1)).squeeze(-1)
-        n, c, h, w = x.shape
-        ohs = torch.arange(oh).view(1, 1, oh, 1) * s[0] + tap // k[1]
-        ows = torch.arange(ow).view(1, 1, 1, ow) * s[1] + tap % k[1]
-        idx = (ohs.clamp_max(h - 1) * w + ows.clamp_max(w - 1)).contiguous()
-        return _nhwc(y.to(BF16)), idx
+        return _nhwc(y.to(BF16)), self._tap_to_plane(tap, k, s, pw_)
 
     # ------------------------------------------------------------------------------------------ loss
     def softmax_xent(self, x, label, grad_scale, want_grad, want_prob):
         """(loss[1] fp32, dx like x, prob fp32): mean NLL over rows, dx = (p - onehot)·grad_scale/rows
         (csrc/ops/softmax_xent.cu:28-107)."""
-        rows = x.shape[0]
+        rows, c = x.shape
         prob = torch.softmax(x.float(), 1)
-        lab = label.long()
-        picked = prob.gather(1, lab.view(-1, 1)).clamp_min(torch.finfo(torch.float32).tiny)
+        lab = label.long().view(-1, 1)
+        valid = (lab >= 0) & (lab < c)                 # a row whose label is out of range adds 0 to the loss
+        lab = torch.where(valid, lab, torch.zeros_like(lab))
+        picked = torch.where(valid, prob.gather(1, lab).clamp_min(torch.finfo(torch.float32).tiny), torch.ones(()))
         loss = (-picked.log().sum() / rows).reshape(1)
         dx = torch.empty(0, dtype=x.dtype)
         if want_grad:
             g = prob.clone()
-            g.scatter_add_(1, lab.view(-1, 1), torch.full((rows, 1), -1.0))
+            g.scatter_add_(1, lab, -valid.float())
             dx = (g * (grad_scale / rows)).to(x.dtype)
         return loss, dx, (prob if want_prob else torch.empty(0))
 
