@@ -60,8 +60,12 @@ struct ConvGeom {
   FastDiv div_ow, div_ohow, div_cg, div_s, div_lp;
   // fp8 kernels only: dequantisation scales read by the epilogue (device memory, so a captured graph sees each step's
   // values).  Kept last so that the kernel-parameter offsets of every other field stay those of the bf16 kernels.
-  const float* scale_x;     // one float: the activation (fprop) / dY (dgrad) scale
-  const float* scale_w;     // per output column of this group (output channel / input channel)
+  const float* scale_x;     // one float: the activation (fprop) / dY (dgrad, wgrad) scale
+  const float* scale_w;     // per output column of this group (output channel / input channel); wgrad: one float, X's
+  // fp8 weight gradient only: the operands are [C][H][W * Np] (batch innermost); one k block is 128 bytes of a row:
+  // 128 / Np columns (Np <= 128) or 128 images of one column (Np a multiple of 128).  The reduction walks (output row,
+  // column run, image chunk): wg_owr column runs of wg_wr columns per row, wg_nch image chunks per run.
+  int wg_np, wg_wr, wg_nch, wg_owr;
 };
 
 // Builds the row table (one thread per row).

@@ -26,6 +26,8 @@ void encode_tmap_bf16_3d(CUtensorMap* map, const void* base, int64_t d0, int64_t
                          int box0, int box1, int box2);
 void splitk_reduce(const at::Tensor& ws, int splits, float* out, long ldo, int M, int N, bool accumulate,
                    cudaStream_t stream);
+void encode_tmap_u8_3d(CUtensorMap* map, const void* base, int64_t d0, int64_t d1, int64_t d2, int64_t stride1,
+                       int64_t stride2, int box2);
 
 static int g_conv_im2col = 1;      // TMA im2col-mode operand fetch where the geometry allows it (C_g % 64 == 0)
 
@@ -38,7 +40,8 @@ extern int g_no_bulk_epi;
 template <int BN, bool A_MN, bool B_MN, int EPI, int GATHER, int CG = 1, typename T = __nv_bfloat16>
 static void launch_conv(const TmapSet& tm, const GemmParams& p, const ConvGeom& cg, int grid, cudaStream_t stream) {
   auto kern = [] {
-    if constexpr (std::is_same<T, __nv_fp8_e5m2>::value) return wgmma_fp8_dgrad_kernel<BN, CG>;
+    if constexpr (GATHER == TILED_WGRAD) return wgmma_fp8_wgrad_kernel<BN, CG>;
+    else if constexpr (std::is_same<T, __nv_fp8_e5m2>::value) return wgmma_fp8_dgrad_kernel<BN, CG>;
     else if constexpr (sizeof(T) == 1) return wgmma_fp8_conv_kernel<BN, CG>;
     else return wgmma_gemm_kernel<BN, A_MN, B_MN, EPI, GATHER, CG>;
   }();
@@ -775,6 +778,117 @@ void conv_wgrad(const at::Tensor& x, const at::Tensor& dy, at::Tensor dw, at::In
   }
 }
 
+// dw[Cout, R*S*Cg] fp32 += alpha * s_dy * s_x * dY8ᵀ · im2col(X8ᵀ) for stride-1 convolutions, with e5m2 dY and e4m3 X in
+// batch-innermost CHWN copies (fp8_quant.cu):
+//   dy8t : e5m2 [Cout][OH][OW][Np];  x8t : e4m3 [Cin][H][W][Np] (Np = 16, 32, 64 or a multiple of 128; pad images zero);
+//   s_dy, s_x : one float each;  cgk : per-tap column slots of the reduction's B side (>= Cg, a multiple of 64: every
+//   64-column chunk is one tap), dropped again by the epilogue.
+// Both copies are read as [C][H][W * Np]: a k block is 128 contiguous bytes of one row, i.e. 128 / Np columns x Np images
+// (Np <= 128) or 128 images of one column, fetched as plain tiled 3-D boxes of dense 128-byte rows; the TMA's zero fill
+// of out-of-range coordinates supplies the spatial padding.  Split-K as in conv_wgrad (partials in a workspace, summed in
+// split order, no atomics); single CTAs or CTA pairs along Cout.
+void conv_wgrad_fp8(const at::Tensor& dy8t, const at::Tensor& x8t, const at::Tensor& s_dy, const at::Tensor& s_x,
+                    at::Tensor dw, at::IntArrayRef kernel, at::IntArrayRef pad, int64_t groups, double alpha, int64_t cgk) {
+  TORCH_CHECK(dy8t.is_cuda() && dy8t.scalar_type() == at::kFloat8_e5m2 && dy8t.dim() == 4 && dy8t.is_contiguous(),
+              "conv_wgrad_fp8: contiguous e5m2 dy8t [Cout, OH, OW, Np] expected");
+  TORCH_CHECK(x8t.is_cuda() && x8t.scalar_type() == at::kFloat8_e4m3fn && x8t.dim() == 4 && x8t.is_contiguous(),
+              "conv_wgrad_fp8: contiguous e4m3 x8t [Cin, H, W, Np] expected");
+  TORCH_CHECK(x8t.device() == dy8t.device(), "conv_wgrad_fp8: operands on different devices");
+  TORCH_CHECK(s_dy.is_cuda() && s_dy.scalar_type() == at::kFloat && s_dy.numel() == 1, "conv_wgrad_fp8: s_dy must be one float");
+  TORCH_CHECK(s_x.is_cuda() && s_x.scalar_type() == at::kFloat && s_x.numel() == 1, "conv_wgrad_fp8: s_x must be one float");
+  TORCH_CHECK(dw.is_cuda() && dw.scalar_type() == at::kFloat && dw.dim() == 2 && dw.is_contiguous(),
+              "conv_wgrad_fp8: contiguous fp32 dw [Cout, R*S*Cg] expected");
+  TORCH_CHECK(kernel.size() == 2 && pad.size() == 2, "conv_wgrad_fp8: kernel and pad take two values");
+  TORCH_CHECK(g_conv_cluster == 1, "conv_wgrad_fp8: the gather multicast-cluster schedule (set_conv_cluster) is bf16-only");
+  TORCH_CHECK(g_conv_mcast == 1, "conv_wgrad_fp8: the im2col multicast-cluster schedule (set_conv_mcast) is bf16-only");
+  const int R = static_cast<int>(kernel[0]), S = static_cast<int>(kernel[1]);
+  const int ph = static_cast<int>(pad[0]), pw = static_cast<int>(pad[1]);
+  TORCH_CHECK(R >= 1 && S >= 1 && R <= 15 && S <= 15, "conv_wgrad_fp8: kernel extents from 1 to 15 are supported");
+  TORCH_CHECK(ph >= 0 && pw >= 0 && ph < R && pw < S, "conv_wgrad_fp8: padding must be below the kernel extent");
+  const int64_t Np = x8t.size(3), Cin = x8t.size(0), H = x8t.size(1), W = x8t.size(2);
+  const int64_t Cout = dy8t.size(0), OH = dy8t.size(1), OW = dy8t.size(2);
+  TORCH_CHECK(dy8t.size(3) == Np && (Np == 16 || Np == 32 || Np == 64 || (Np > 0 && Np % 128 == 0)),
+              "conv_wgrad_fp8: both copies need the same Np: 16, 32, 64 or a multiple of 128");
+  TORCH_CHECK(OH == H + 2 * ph - R + 1 && OW == W + 2 * pw - S + 1 && OH >= 1 && OW >= 1,
+              "conv_wgrad_fp8: dY extent is not that of a stride-1 convolution over H x W");
+  TORCH_CHECK(groups >= 1 && Cin % groups == 0 && Cout % groups == 0, "conv_wgrad_fp8: channel counts");
+  const int Cg = static_cast<int>(Cin / groups), Cout_g = static_cast<int>(Cout / groups);
+  TORCH_CHECK(Cg % 8 == 0 && Cout_g % 8 == 0, "conv_wgrad_fp8: channels per group must be multiples of 8");
+  TORCH_CHECK(cgk >= Cg && cgk % 64 == 0, "conv_wgrad_fp8: per-tap slots cgk must be a multiple of 64 and >= Cg");
+  const int64_t k_real = static_cast<int64_t>(R) * S * Cg;
+  TORCH_CHECK(dw.size(0) == Cout && dw.size(1) == k_real, "conv_wgrad_fp8: dw shape mismatch");
+  const int wr = Np < 128 ? static_cast<int>(128 / Np) : 1, nch = Np < 128 ? 1 : static_cast<int>(Np / 128);
+  const int owr = static_cast<int>((OW + wr - 1) / wr);
+  const int64_t kb = OH * owr * nch;
+  TORCH_CHECK(kb < (1L << 31) && static_cast<int64_t>(R) * S * cgk < (1L << 31) && (W + 16) * Np < (1L << 31) &&
+              Cin * H * W * Np < (1L << 40), "conv_wgrad_fp8: problem too large");
+  ConvGeom cg{};
+  cg.Cg = Cg;
+  cg.Cgk = static_cast<int>(cgk);
+  cg.R = R; cg.S = S;
+  cg.sh = 1; cg.sw = 1;
+  cg.off_h = -ph; cg.off_w = -pw;
+  cg.dr = 1;
+  cg.K = static_cast<int>(R * S * cgk);
+  cg.div_cg = make_fastdiv(static_cast<uint32_t>(cgk));
+  cg.div_s = make_fastdiv(S);
+  cg.scale_x = s_dy.data_ptr<float>();
+  cg.scale_w = s_x.data_ptr<float>();
+  cg.wg_np = static_cast<int>(Np); cg.wg_wr = wr; cg.wg_nch = nch; cg.wg_owr = owr;
+  c10::cuda::CUDAGuard guard(dy8t.device());
+  auto stream = at::cuda::getCurrentCUDAStream();
+  const int sms = at::cuda::getCurrentDeviceProperties()->multiProcessorCount;
+  // tile width: 128 unless that pads the columns by more than an eighth
+  const int bn = (cg.K + 127L) / 128 * 128 * 8 <= cg.K * 9L ? 128 : 64;
+  const long m_blocks = (Cout_g + BLOCK_M - 1) / BLOCK_M, n_blocks = (cg.K + bn - 1) / bn;
+  const long tiles = m_blocks * n_blocks;
+  long split = std::max<long>(1, (2L * sms + tiles - 1) / tiles);
+  split = std::min<long>(split, std::max<long>(1, kb / 8));
+  const bool pair = g_conv_pair && pair_cta_enabled() && m_blocks >= 2 && m_blocks % 2 == 0;
+  // every group's tensor maps are encoded before any device work
+  std::vector<TmapSet> maps(groups);
+  for (int gidx = 0; gidx < groups; ++gidx) {
+    const uint8_t* a = reinterpret_cast<const uint8_t*>(dy8t.data_ptr()) + gidx * Cout_g * OH * OW * Np;
+    const uint8_t* b = reinterpret_cast<const uint8_t*>(x8t.data_ptr()) + gidx * Cg * H * W * Np;
+    encode_tmap_u8_3d(&maps[gidx].a[0], a, OW * Np, OH, Cout_g, OW * Np, OH * OW * Np, BLOCK_M);
+    encode_tmap_u8_3d(&maps[gidx].b[0], b, W * Np, H, Cg, W * Np, H * W * Np, std::min(64, bn / (pair ? 2 : 1)));
+  }
+  for (int gidx = 0; gidx < groups; ++gidx) {
+    GemmParams p{};
+    p.max_stages = g_max_stages;
+    p.no_bulk_epi = g_no_bulk_epi;
+    p.cluster = 1;
+    p.M = Cout_g;
+    p.N = cg.K;
+    p.kb_per_src = static_cast<int>(kb);
+    p.num_src = 1;
+    p.split_k = static_cast<int>(split);
+    p.c_f32 = dw.data_ptr<float>() + static_cast<long>(gidx) * Cout_g * k_real;
+    p.ldc = k_real;
+    if (cgk != Cg) { p.col_cg = Cg; p.col_cgk = static_cast<int>(cgk); }
+    p.atomic = 1;
+    p.alpha = static_cast<float>(alpha);
+    float* const dwg = p.c_f32;
+    at::Tensor ws;
+    if (split > 1) {
+      ws = at::empty({split, Cout_g, k_real}, dw.options());
+      p.c_f32 = ws.data_ptr<float>();
+      p.split_stride = static_cast<long>(Cout_g) * k_real;
+      p.atomic = 0;
+    }
+    if (pair) {
+      const int grid = pair_grid(m_blocks, n_blocks, split, sms);
+      if (bn == 64) launch_conv<64, false, false, EPI_F32, TILED_WGRAD, 2, __nv_fp8_e5m2>(maps[gidx], p, cg, grid, stream);
+      else launch_conv<128, false, false, EPI_F32, TILED_WGRAD, 2, __nv_fp8_e5m2>(maps[gidx], p, cg, grid, stream);
+    } else {
+      const int grid = static_cast<int>(std::max<long>(1, std::min<long>(tiles * split, sms)));
+      if (bn == 64) launch_conv<64, false, false, EPI_F32, TILED_WGRAD, 1, __nv_fp8_e5m2>(maps[gidx], p, cg, grid, stream);
+      else launch_conv<128, false, false, EPI_F32, TILED_WGRAD, 1, __nv_fp8_e5m2>(maps[gidx], p, cg, grid, stream);
+    }
+    if (split > 1) splitk_reduce(ws, static_cast<int>(split), dwg, k_real, Cout_g, static_cast<int>(k_real), true, stream);
+  }
+}
+
 // Pack the dgrad operand from the fp32 master weights: w [Cout][R][S][Cg] -> wt [groups][Cg][R][S][Cop] bf16, where
 // Cop >= Cout_g is the per-tap slot count (Cout_g rounded up to 64 on the channel-padded im2col path; pad = 0).
 __global__ void pack_dgrad_kernel(const float* __restrict__ w, __nv_bfloat16* __restrict__ wt, int Cout, int RS, int Cg,
@@ -866,6 +980,8 @@ TORCH_LIBRARY_FRAGMENT(poseidon, m) {
         "-> Tensor", &psd::conv_dgrad_w);
   m.def("conv_wgrad(Tensor x, Tensor dy, Tensor(a!) dw, int[] kernel, int[] stride, int[] pad, int groups, int mode, "
         "float alpha, int cgk) -> ()", &psd::conv_wgrad);
+  m.def("conv_wgrad_fp8(Tensor dy8t, Tensor x8t, Tensor s_dy, Tensor s_x, Tensor(a!) dw, int[] kernel, int[] pad, "
+        "int groups, float alpha, int cgk) -> ()", &psd::conv_wgrad_fp8);
   m.def("conv_pack_dgrad(Tensor w, int Cout, int RS, int Cg, int groups, Tensor? out, int cop) -> Tensor", &psd::conv_pack_dgrad);
   m.def("conv_pack_padded(Tensor wb, int Cout, int RS, int Cg, int Cgk, Tensor? out) -> Tensor", &psd::conv_pack_padded);
 }

@@ -64,6 +64,22 @@ void encode_tmap_bf16_3d(CUtensorMap* map, const void* base, int64_t d0, int64_t
   TORCH_CHECK(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled (3-D) failed: ", static_cast<int>(r));
 }
 
+// 3-D 8-bit tensor map [d2][d1][d0] (d0 contiguous), 128B swizzle, boxes of {128 bytes, 1, box2}: the fp8 weight-gradient
+// operands [C][H][W * Np].  strides in bytes.
+void encode_tmap_u8_3d(CUtensorMap* map, const void* base, int64_t d0, int64_t d1, int64_t d2, int64_t stride1,
+                       int64_t stride2, int box2) {
+  TORCH_CHECK((reinterpret_cast<uintptr_t>(base) & 15) == 0 && stride1 % 16 == 0 && stride2 % 16 == 0,
+              "3-D TMA map: 16-byte alignment of base and strides");
+  cuuint64_t dims[3] = {static_cast<cuuint64_t>(d0), static_cast<cuuint64_t>(d1), static_cast<cuuint64_t>(d2)};
+  cuuint64_t strides[2] = {static_cast<cuuint64_t>(stride1), static_cast<cuuint64_t>(stride2)};
+  cuuint32_t box[3] = {128, 1, static_cast<cuuint32_t>(box2)};
+  cuuint32_t estr[3] = {1, 1, 1};
+  CUresult r = get_encode_fn()(map, CU_TENSOR_MAP_DATA_TYPE_UINT8, 3, const_cast<void*>(base), dims, strides, box, estr,
+                               CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                               CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  TORCH_CHECK(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled (3-D, 8-bit) failed");
+}
+
 // 4-D im2col-mode tensor map over an NHWC tensor (channels innermost, pixel pitch `pitch` elements).
 //   lower / upper : bounding-box corner offsets {w, h} (cuTensorMapEncodeIm2col semantics: base pixels run from
 //                   `lower` to `extent + upper - 1` in steps of the traversal stride)

@@ -40,7 +40,9 @@ constexpr int kGatherThreads = 128;
 constexpr int kGatherMaxBN = 128;
 // GATHER_A / GATHER_B: operand built by the cp.async gather warps (any channel count, ROW mode).
 // IM2COL_A / IM2COL_B: operand fetched by the TMA engine in im2col mode (C_g % 64 == 0): no gather warps at all.
-enum GatherMode : int { GATHER_NONE = 0, GATHER_A = 1, GATHER_B = 2, IM2COL_A = 3, IM2COL_B = 4 };
+// TILED_WGRAD: the fp8 weight gradient over batch-innermost CHWN copies — both operands K-major plain tiled 3-D boxes,
+// the producer decoding each k block into (output row, column run, image chunk) (see wgmma_fp8_wgrad_kernel).
+enum GatherMode : int { GATHER_NONE = 0, GATHER_A = 1, GATHER_B = 2, IM2COL_A = 3, IM2COL_B = 4, TILED_WGRAD = 5 };
 __host__ __device__ constexpr bool has_gather_warps(int g) { return g == GATHER_A || g == GATHER_B; }
 
 enum EpiMode : int { EPI_BF16 = 0, EPI_F32 = 1, EPI_SGD = 2 };
@@ -388,8 +390,10 @@ __device__ __forceinline__ void wgmma_gemm_body(const TmapSet& tm, const GemmPar
   constexpr int KB = 128 / static_cast<int>(sizeof(TA));    // elements per k block
   static_assert(sizeof(TA) == sizeof(TB), "both operands bf16, or both fp8");
   static_assert(!kFp8 || std::is_same<TB, __nv_fp8_e4m3>::value, "fp8 B operand: e4m3");
-  static_assert(!kFp8 || (GATHER == IM2COL_A && !A_MN && !B_MN && EPI == EPI_BF16 && BN <= 128),
-                "fp8 operands: K-major im2col convolution with the bf16 epilogue only");
+  static_assert(!kFp8 || (!A_MN && !B_MN && BN <= 128 &&
+                          ((GATHER == IM2COL_A && EPI == EPI_BF16) || (GATHER == TILED_WGRAD && EPI == EPI_F32))),
+                "fp8 operands: K-major im2col convolution with the bf16 epilogue, or the tiled weight gradient (fp32)");
+  static_assert(GATHER != TILED_WGRAD || kFp8, "the tiled weight-gradient producer reads fp8 CHWN copies");
   static_assert(CG == 1 || CG == 2, "one CTA or a CTA pair per B tile");
   static_assert(CG == 1 || !has_gather_warps(GATHER), "CTA pairs share a TMA-fetched B tile");
   static_assert(!has_gather_warps(GATHER) || BN <= kGatherMaxBN, "gather kernels: accumulator register budget");
@@ -494,6 +498,28 @@ __device__ __forceinline__ void wgmma_gemm_body(const TmapSet& tm, const GemmPar
             im_offw[c] = static_cast<uint16_t>(tap - r * cg.S);
           }
         }
+        // TILED_WGRAD: k block g0 -> (output row, column run, image chunk), then advanced incrementally; per B box of
+        // this CTA (rows [prank * BN/CG, ...) of the tile, kRowsB each) its tap displacement and first channel
+        constexpr int kRowsB = BN / CG < 64 ? BN / CG : 64;       // rows per B box: 64 columns of one tap, or half
+        constexpr int kBoxesB = GATHER == TILED_WGRAD ? BN / CG / kRowsB : 1;
+        [[maybe_unused]] int wg_n = 0, wg_w = 0, wg_h = 0, wg_dw[kBoxesB], wg_dh[kBoxesB], wg_c[kBoxesB];
+        if constexpr (GATHER == TILED_WGRAD) {
+          wg_n = g0 % cg.wg_nch;
+          const int rest = g0 / cg.wg_nch;
+          wg_w = rest % cg.wg_owr;
+          wg_h = rest / cg.wg_owr;
+#pragma unroll
+          for (int j = 0; j < kBoxesB; ++j) {
+            const int row0 = prank * (BN / CG) + j * kRowsB;
+            int kc = n_blk * BN + (row0 & ~63);
+            if (kc >= cg.K) kc = 0;                      // columns past K are dropped by the epilogue: load anything valid
+            const int tap = static_cast<int>(fdiv(static_cast<uint32_t>(kc), cg.div_cg));
+            const int r = static_cast<int>(fdiv(static_cast<uint32_t>(tap), cg.div_s));
+            wg_c[j] = kc - tap * cg.Cgk + (row0 & 63);
+            wg_dh[j] = r + im_org_h;
+            wg_dw[j] = tap - r * cg.S + im_org_w;
+          }
+        }
         // (source, k-block) advance incrementally: no divisions in the single-thread producer loop
         int src_lin = g0 / p.kb_per_src;
         int kb = g0 - src_lin * p.kb_per_src;
@@ -572,6 +598,23 @@ __device__ __forceinline__ void wgmma_gemm_body(const TmapSet& tm, const GemmPar
               }
             }
             TmaProducer<BN, A_MN, B_MN, CG>::load_a(tm, src, kb, m_blk, sa32, fbar);
+          } else if constexpr (GATHER == TILED_WGRAD) {
+            // One k block = 128 bytes of the (column, image) row of output row wg_h, starting at column w0, image n0.
+            // A = dYᵀ rows (output channels): box {128 B, 1, 128 co} of [Cout_g][OH][OW * Np]; columns past OW and
+            // channels past Cout_g are zero-filled, so a partial last column run adds nothing.
+            // B = X rows (tap, ci): per 64-column chunk, a box {128 B, 1, rows} of [Cg][H][W * Np] displaced by the tap;
+            // the zero fill outside the image (negative or past-the-end coordinates) is the convolution's padding.
+            // CTA pairs: this CTA fetches rows [prank * BN/2, (prank + 1) * BN/2) of the B tile for both.
+            const int x0 = wg_w * cg.wg_wr * cg.wg_np + wg_n * 128;
+            mbar_arrive_expect_tx(&full_bar[stage], S::kStageBytes);
+            tma_load_3d_u32(sa32, &tm.a[0], fbar, x0, wg_h, m_blk * BLOCK_M);
+#pragma unroll
+            for (int j = 0; j < kBoxesB; ++j) {
+              const uint32_t dst = sb32 + (prank * (BN / CG) + j * kRowsB) * 128;
+              const int xb = x0 + wg_dw[j] * cg.wg_np;
+              if constexpr (CG == 2) tma_load_3d_mcast_u32(dst, &tm.b[0], fbar, xb, wg_h + wg_dh[j], wg_c[j], 0x3);
+              else tma_load_3d_u32(dst, &tm.b[0], fbar, xb, wg_h + wg_dh[j], wg_c[j]);
+            }
           } else if constexpr (GATHER == GATHER_A) {
             mbar_arrive_expect_tx(&full_bar[stage], S::kBBytes);     // the whole B tile lands here (C slices)
             if (C == 1) {
@@ -597,6 +640,12 @@ __device__ __forceinline__ void wgmma_gemm_body(const TmapSet& tm, const GemmPar
           }
           }  // elect_one
           __syncwarp();
+          if constexpr (GATHER == TILED_WGRAD) {
+            if (++wg_n == cg.wg_nch) {
+              wg_n = 0;
+              if (++wg_w == cg.wg_owr) { wg_w = 0; ++wg_h; }
+            }
+          }
           if (++stage == nst) { stage = 0; phase ^= 1; }
           if (++kb == p.kb_per_src) {
             kb = 0;
@@ -731,6 +780,9 @@ __device__ __forceinline__ void wgmma_gemm_body(const TmapSet& tm, const GemmPar
       wgmma_wait<0>();
       wgmma_fence_regs(acc);
       if (prev >= 0) release(prev);
+      // fp8 weight gradient: the fp32 epilogue scales by s_dy * s_x * alpha (one scale each, no per-column factor)
+      [[maybe_unused]] float alpha_w = 0.f;
+      if constexpr (GATHER == TILED_WGRAD) alpha_w = __ldg(cg.scale_x) * __ldg(cg.scale_w) * p.alpha;
 
       const int col0 = n_blk * BN;
       [[maybe_unused]] float* const c_f32 = p.c_f32 + (p.split_stride > 0 ? split * p.split_stride : 0);   // this split's slice
@@ -760,7 +812,7 @@ __device__ __forceinline__ void wgmma_gemm_body(const TmapSet& tm, const GemmPar
 #pragma unroll 1
             for (int qq = 0; qq < 4; ++qq) {
               if ((e >> 1) == qq) {
-                frag_to_slab<BN, LDS>(acc, epi_stage, (e & 1) * 16, lane, p.alpha);
+                frag_to_slab<BN, LDS>(acc, epi_stage, (e & 1) * 16, lane, GATHER == TILED_WGRAD ? alpha_w : p.alpha);
                 fence_proxy_async_smem();               // generic-proxy writes -> visible to the bulk-copy engine
               }
               epi_bar_sync();
@@ -851,8 +903,8 @@ __device__ __forceinline__ void wgmma_gemm_body(const TmapSet& tm, const GemmPar
 #pragma unroll
                 for (int h = 0; h < 2; ++h) {
                   float* dst = stage_w + ((lane >> 2) + 8 * h) * 33 + 8 * i + 2 * (lane & 3);
-                  dst[0] = acc[4 * (4 * c + i) + 2 * h] * p.alpha;
-                  dst[1] = acc[4 * (4 * c + i) + 2 * h + 1] * p.alpha;
+                  dst[0] = acc[4 * (4 * c + i) + 2 * h] * (GATHER == TILED_WGRAD ? alpha_w : p.alpha);
+                  dst[1] = acc[4 * (4 * c + i) + 2 * h + 1] * (GATHER == TILED_WGRAD ? alpha_w : p.alpha);
                 }
               }
               __syncwarp();
@@ -890,6 +942,15 @@ template <int BN, int CG>
 __global__ void __launch_bounds__(kNumThreads, 1)
 wgmma_fp8_dgrad_kernel(const __grid_constant__ TmapSet tm, const GemmParams p, const ConvGeom cg) {
   wgmma_gemm_body<BN, false, false, EPI_BF16, IM2COL_A, CG, __nv_fp8_e5m2, __nv_fp8_e4m3>(tm, p, cg);
+}
+
+// e5m2 dY x e4m3 X: the stride-1 weight gradient (conv_wgrad_fp8).  Rows = output channels, columns = (tap, ci), the
+// reduction runs over pixels with the batch innermost, read from CHWN copies as plain tiled boxes (TILED_WGRAD); fp32
+// epilogue (split-K partials / add onto dw) scaled by s_dy * s_x * alpha.
+template <int BN, int CG>
+__global__ void __launch_bounds__(kNumThreads, 1)
+wgmma_fp8_wgrad_kernel(const __grid_constant__ TmapSet tm, const GemmParams p, const ConvGeom cg) {
+  wgmma_gemm_body<BN, false, false, EPI_F32, TILED_WGRAD, CG, __nv_fp8_e5m2, __nv_fp8_e4m3>(tm, p, cg);
 }
 
 // Persistent kernels on clusters: a grid holding more clusters than the GPU can run at once would leave its last clusters

@@ -10,6 +10,10 @@
 //   fp8_quant_weight_dgrad : fp32 master -> e4m3 in conv_pack_dgrad's order, [groups*Cg][R*S*Cok] (input-channel rows,
 //                      K = (tap, co), slots >= Cout_g zero), one scale per input channel: the input channel is the output
 //                      column of the data gradient, so its scale factors out of the accumulation.
+//   fp8_quant_act_t / fp8_quant_grad_t : the weight gradient's batch-innermost copies [C][H][W][Np] of X (e4m3) and
+//                      dY (e5m2), Np = N rounded up to 16, 32, 64 or a multiple of 128 (a 128-byte row then holds whole
+//                      columns or whole image chunks), pad images zero; scale rules, mask and kernels as fp8_quant_act /
+//                      fp8_quant_grad.
 //
 // Scaling is just in time: s = MAX / amax(|v|) (MAX = 448 for e4m3, 57344 for e5m2; 1 when amax == 0),
 // q = cvt.rn.satfinite(v * s), and 1 / s is stored for the GEMM epilogue.  amax uses fmaxf, which skips NaN, so a NaN
@@ -229,49 +233,180 @@ __global__ void __launch_bounds__(kQuantThreads) quant_weight_dgrad_kernel(const
   }
 }
 
-// dy: bf16 NHWC (logical [N, C, H, W], pixel pitch >= C); s_out: one float, receives 1 / s (s = 57344 / amax).
-// y (optional): the layer's forward output (same logical shape, any pixel pitch): dY is first masked as relu_bwd does it.
-// Returns (e5m2 [N, C, H, W] as a channel slice of a channels-last [N, round16(C), H, W] tensor, the bf16 dY the cast read:
-// `dy` itself, or the masked dense copy).
-std::tuple<at::Tensor, at::Tensor> fp8_quant_grad(const at::Tensor& dy, at::Tensor s_out, const c10::optional<at::Tensor>& y,
-                                                  double slope) {
-  TORCH_CHECK(dy.is_cuda() && dy.scalar_type() == at::kBFloat16, "fp8_quant_grad: bf16 CUDA dY expected");
-  TORCH_CHECK(s_out.is_cuda() && s_out.scalar_type() == at::kFloat && s_out.numel() == 1 && s_out.is_contiguous(),
-              "fp8_quant_grad: s_out must be one fp32 element");
-  c10::cuda::CUDAGuard guard(dy.device());
-  const NhwcView dv = nhwc_view(dy);
-  TORCH_CHECK(dv.C % 8 == 0 && dv.pitch % 8 == 0 && (reinterpret_cast<uintptr_t>(dy.data_ptr()) & 15) == 0,
-              "fp8_quant_grad: channels and pixel pitch must be multiples of 8 (16-byte vectors)");
-  NhwcView yv{};
-  if (y.has_value()) {
-    TORCH_CHECK(y->is_cuda() && y->scalar_type() == at::kBFloat16, "fp8_quant_grad: bf16 CUDA mask y expected");
-    yv = nhwc_view(*y);
-    TORCH_CHECK(yv.N == dv.N && yv.C == dv.C && yv.H == dv.H && yv.W == dv.W && yv.pitch % 8 == 0 &&
-                (reinterpret_cast<uintptr_t>(y->data_ptr()) & 15) == 0, "fp8_quant_grad: y must match dY (pitch a multiple of 8)");
+// Cast-transpose into the batch-innermost copy of the fp8 weight gradient: bf16 NHWC x (pixel pitch >= C) ->
+// yt [C][H][W][Np] (images N..Np-1 zero, Np a multiple of 16), with the scale rule of cast_fp8_nhwc_kernel (the same partial maxima give the
+// same s, and every element is cast on its own, so yt is bit for bit the transpose of that kernel's output).  y (optional)
+// also receives the dense NHWC copy of cast_fp8_nhwc_kernel (pixel pitch pitch8, pad channels zero), so one read of x
+// serves both.  One CTA per (pixel, 64-channel slab, 32-image slab); the tile turns around in shared memory so that
+// both sides move whole 16- / 8-byte pieces.
+constexpr int kTileN = 32, kTileC = 64;
+
+// Images per channel row of the batch-innermost copies: 16, 32, 64, or a multiple of 128 (conv_wgrad_fp8).
+static int chwn_images(int n) {
+  if (n <= 64) return n <= 16 ? 16 : (n <= 32 ? 32 : 64);
+  return (n + 127) / 128 * 128;
+}
+template <typename F>
+__global__ void __launch_bounds__(kQuantThreads) cast_fp8_chwn_kernel(const __nv_bfloat16* __restrict__ x, int N, int Np, int C,
+                                                                      int HW, long pitch, const float* __restrict__ partial,
+                                                                      int nparts, uint8_t* __restrict__ yt,
+                                                                      uint8_t* __restrict__ y, int pitch8,
+                                                                      float* __restrict__ s_out) {
+  __shared__ float red[kQuantThreads / 32];
+  __shared__ __align__(16) uint8_t tile[kTileC][kTileN];
+  float m = 0.f;
+  for (int i = threadIdx.x; i < nparts; i += blockDim.x) m = fmaxf(m, partial[i]);
+  const float s = quant_scale<F>(block_max(m, red));
+  if (blockIdx.x == 0 && blockIdx.y == 0 && blockIdx.z == 0 && threadIdx.x == 0) *s_out = 1.f / s;
+  const int hw = blockIdx.x, c0 = blockIdx.y * kTileC, n0 = blockIdx.z * kTileN;
+  {
+    const int n = threadIdx.x / 8, v = threadIdx.x % 8;          // image n0 + n, channels c0 + 8v ..
+    const int nn = n0 + n, c = c0 + 8 * v;
+    uint32_t lo = 0, hi = 0;
+    if (nn < N && c < C) {
+      float a[8];
+      unpack8(ld8(x + (static_cast<long>(nn) * HW + hw) * pitch + c), a);
+      lo = cvt_fp8x2<F>(a[0] * s, a[1] * s) | (cvt_fp8x2<F>(a[2] * s, a[3] * s) << 16);
+      hi = cvt_fp8x2<F>(a[4] * s, a[5] * s) | (cvt_fp8x2<F>(a[6] * s, a[7] * s) << 16);
+    }
+    if (y != nullptr && nn < N && c < pitch8)                     // channels [C, pitch8): the zero pad
+      *reinterpret_cast<uint2*>(y + (static_cast<long>(nn) * HW + hw) * pitch8 + c) = make_uint2(lo, hi);
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      tile[8 * v + k][n] = static_cast<uint8_t>(lo >> (8 * k));
+      tile[8 * v + 4 + k][n] = static_cast<uint8_t>(hi >> (8 * k));
+    }
   }
-  const int pitch8 = (dv.C + 15) / 16 * 16;
-  at::Tensor full = empty_nhwc(dv.N, pitch8, dv.H, dv.W, dy.options().dtype(at::kFloat8_e5m2));
+  __syncthreads();
+  const int c = threadIdx.x / 4, n8 = (threadIdx.x % 4) * 8;     // Np % 16 == 0: a run of 8 images is all in or all out
+  if (c0 + c < C && n0 + n8 < Np)
+    *reinterpret_cast<uint2*>(yt + (static_cast<long>(c0 + c) * HW + hw) * Np + n0 + n8) =
+        *reinterpret_cast<const uint2*>(&tile[c][n8]);
+}
+
+static void launch_cast_chwn(const at::Tensor& x, const NhwcView& xv, long pitch, int Np, const at::Tensor& partial,
+                                  at::Tensor& yt, at::Tensor* y, int pitch8, at::Tensor& s_out, bool e5m2) {
+  const dim3 grid(static_cast<unsigned>(xv.H * xv.W), static_cast<unsigned>((xv.C + kTileC - 1) / kTileC),
+                  static_cast<unsigned>((Np + kTileN - 1) / kTileN));
+  auto stream = at::cuda::getCurrentCUDAStream();
+  const auto* xp = reinterpret_cast<const __nv_bfloat16*>(x.data_ptr());
+  uint8_t* yp = y != nullptr ? reinterpret_cast<uint8_t*>(y->data_ptr()) : nullptr;
+  if (e5m2)
+    cast_fp8_chwn_kernel<E5M2><<<grid, kQuantThreads, 0, stream>>>(
+        xp, xv.N, Np, xv.C, xv.H * xv.W, pitch, partial.data_ptr<float>(), static_cast<int>(partial.numel()),
+        reinterpret_cast<uint8_t*>(yt.data_ptr()), yp, pitch8, s_out.data_ptr<float>());
+  else
+    cast_fp8_chwn_kernel<E4M3><<<grid, kQuantThreads, 0, stream>>>(
+        xp, xv.N, Np, xv.C, xv.H * xv.W, pitch, partial.data_ptr<float>(), static_cast<int>(partial.numel()),
+        reinterpret_cast<uint8_t*>(yt.data_ptr()), yp, pitch8, s_out.data_ptr<float>());
+  C10_CUDA_KERNEL_LAUNCH_CHECK();
+}
+
+// x: bf16 NHWC (pitched: concat-slab slices too); s_out: one float, receives 1 / s with fp8_quant_act's rule.
+// Returns e4m3 [C, H, W, chwn_images(N)], images N.. zero: the weight gradient's copy of the forward operand.
+at::Tensor fp8_quant_act_t(const at::Tensor& x, at::Tensor s_out) {
+  TORCH_CHECK(x.is_cuda() && x.scalar_type() == at::kBFloat16, "fp8_quant_act_t: bf16 CUDA input expected");
+  TORCH_CHECK(s_out.is_cuda() && s_out.scalar_type() == at::kFloat && s_out.numel() == 1 && s_out.is_contiguous(),
+              "fp8_quant_act_t: s_out must be one fp32 element");
+  c10::cuda::CUDAGuard guard(x.device());
+  const NhwcView xv = nhwc_view(x);
+  TORCH_CHECK(xv.C % 8 == 0 && xv.pitch % 8 == 0 && (reinterpret_cast<uintptr_t>(x.data_ptr()) & 15) == 0,
+              "fp8_quant_act_t: channels and pixel pitch must be multiples of 8 (16-byte vectors)");
+  TORCH_CHECK(static_cast<long>(xv.H) * xv.W < (1L << 31), "fp8_quant_act_t: too many pixels per image");
+  const int Np = chwn_images(xv.N);
+  at::Tensor xt = at::empty({xv.C, xv.H, xv.W, Np}, x.options().dtype(at::kFloat8_e4m3fn));
+  const long pixels = static_cast<long>(xv.N) * xv.H * xv.W;
+  const int blocks = grid_for(pixels * (xv.C / 8), kQuantThreads, kAmaxMaxBlocks);
+  at::Tensor partial = at::empty({blocks}, x.options().dtype(at::kFloat));
+  amax_nhwc_kernel<<<blocks, kQuantThreads, 0, at::cuda::getCurrentCUDAStream()>>>(
+      reinterpret_cast<const __nv_bfloat16*>(x.data_ptr()), pixels, xv.C, xv.pitch, partial.data_ptr<float>());
+  C10_CUDA_KERNEL_LAUNCH_CHECK();
+  launch_cast_chwn(x, xv, xv.pitch, Np, partial, xt, nullptr, 0, s_out, false);
+  return xt;
+}
+
+// amax pass of the dY quantisers: over dy itself, or (y given) over dy masked by the layer's own ReLU backward, written
+// dense into *src.  Returns the partial maxima; *src / *src_pitch: the bf16 dY the cast pass reads.
+static at::Tensor grad_amax(const at::Tensor& dy, const NhwcView& dv, const c10::optional<at::Tensor>& y, const NhwcView& yv,
+                            double slope, at::Tensor* src, long* src_pitch) {
   const long pixels = static_cast<long>(dv.N) * dv.H * dv.W;
   auto stream = at::cuda::getCurrentCUDAStream();
   const int blocks = grid_for(pixels * (dv.C / 8), kQuantThreads, kAmaxMaxBlocks);
   at::Tensor partial = at::empty({blocks}, dy.options().dtype(at::kFloat));
-  at::Tensor src = dy;
-  long src_pitch = dv.pitch;
+  *src = dy;
+  *src_pitch = dv.pitch;
   if (y.has_value()) {
-    src = empty_nhwc(dv.N, dv.C, dv.H, dv.W, dy.options());
-    src_pitch = dv.C;
+    *src = empty_nhwc(dv.N, dv.C, dv.H, dv.W, dy.options());
+    *src_pitch = dv.C;
     mask_amax_nhwc_kernel<<<blocks, kQuantThreads, 0, stream>>>(
         reinterpret_cast<const __nv_bfloat16*>(dy.data_ptr()), dv.pitch, reinterpret_cast<const __nv_bfloat16*>(y->data_ptr()),
-        yv.pitch, static_cast<float>(slope), pixels, dv.C, reinterpret_cast<__nv_bfloat16*>(src.data_ptr()),
+        yv.pitch, static_cast<float>(slope), pixels, dv.C, reinterpret_cast<__nv_bfloat16*>(src->data_ptr()),
         partial.data_ptr<float>());
   } else {
     amax_nhwc_kernel<<<blocks, kQuantThreads, 0, stream>>>(reinterpret_cast<const __nv_bfloat16*>(dy.data_ptr()), pixels,
                                                            dv.C, dv.pitch, partial.data_ptr<float>());
   }
   C10_CUDA_KERNEL_LAUNCH_CHECK();
-  cast_fp8_nhwc_kernel<E5M2><<<grid_for(pixels * (pitch8 / 16), kQuantThreads), kQuantThreads, 0, stream>>>(
+  return partial;
+}
+
+// Argument checks of the dY quantisers (before any device work).
+static NhwcView check_grad_args(const at::Tensor& dy, const at::Tensor& s_out, const c10::optional<at::Tensor>& y,
+                                NhwcView* yv) {
+  TORCH_CHECK(dy.is_cuda() && dy.scalar_type() == at::kBFloat16, "fp8 dY quantiser: bf16 CUDA dY expected");
+  TORCH_CHECK(s_out.is_cuda() && s_out.scalar_type() == at::kFloat && s_out.numel() == 1 && s_out.is_contiguous(),
+              "fp8 dY quantiser: s_out must be one fp32 element");
+  const NhwcView dv = nhwc_view(dy);
+  TORCH_CHECK(dv.C % 8 == 0 && dv.pitch % 8 == 0 && (reinterpret_cast<uintptr_t>(dy.data_ptr()) & 15) == 0,
+              "fp8 dY quantiser: channels and pixel pitch must be multiples of 8 (16-byte vectors)");
+  if (y.has_value()) {
+    TORCH_CHECK(y->is_cuda() && y->scalar_type() == at::kBFloat16, "fp8 dY quantiser: bf16 CUDA mask y expected");
+    *yv = nhwc_view(*y);
+    TORCH_CHECK(yv->N == dv.N && yv->C == dv.C && yv->H == dv.H && yv->W == dv.W && yv->pitch % 8 == 0 &&
+                (reinterpret_cast<uintptr_t>(y->data_ptr()) & 15) == 0, "fp8 dY quantiser: y must match dY (pitch a multiple of 8)");
+  }
+  return dv;
+}
+
+// The weight-gradient sibling of fp8_quant_grad (same arguments, scale rule, mask and kernels): one amax pass, then one
+// cast pass that writes the batch-innermost e5m2 copy [C, OH, OW, chwn_images(N)] and, with nhwc, also fp8_quant_grad's NHWC
+// copy (for an fp8 data gradient).  Returns (dy8t, the NHWC copy or an empty tensor, the bf16 dY the cast read).
+std::tuple<at::Tensor, at::Tensor, at::Tensor> fp8_quant_grad_t(const at::Tensor& dy, at::Tensor s_out,
+                                                                const c10::optional<at::Tensor>& y, double slope, bool nhwc) {
+  NhwcView yv{};
+  const NhwcView dv = check_grad_args(dy, s_out, y, &yv);
+  TORCH_CHECK(static_cast<long>(dv.H) * dv.W < (1L << 31), "fp8_quant_grad_t: too many pixels per image");
+  c10::cuda::CUDAGuard guard(dy.device());
+  const int Np = chwn_images(dv.N), pitch8 = (dv.C + 15) / 16 * 16;
+  at::Tensor dyt = at::empty({dv.C, dv.H, dv.W, Np}, dy.options().dtype(at::kFloat8_e5m2));
+  at::Tensor full = nhwc ? empty_nhwc(dv.N, pitch8, dv.H, dv.W, dy.options().dtype(at::kFloat8_e5m2))
+                         : at::empty({0}, dy.options().dtype(at::kFloat8_e5m2));
+  at::Tensor src;
+  long src_pitch = 0;
+  at::Tensor partial = grad_amax(dy, dv, y, yv, slope, &src, &src_pitch);
+  launch_cast_chwn(src, dv, src_pitch, Np, partial, dyt, nhwc ? &full : nullptr, pitch8, s_out, true);
+  return {dyt, nhwc ? full.narrow(1, 0, dv.C) : full, src};
+}
+
+// dy: bf16 NHWC (logical [N, C, H, W], pixel pitch >= C); s_out: one float, receives 1 / s (s = 57344 / amax).
+// y (optional): the layer's forward output (same logical shape, any pixel pitch): dY is first masked as relu_bwd does it.
+// Returns (e5m2 [N, C, H, W] as a channel slice of a channels-last [N, round16(C), H, W] tensor, the bf16 dY the cast read:
+// `dy` itself, or the masked dense copy).
+std::tuple<at::Tensor, at::Tensor> fp8_quant_grad(const at::Tensor& dy, at::Tensor s_out, const c10::optional<at::Tensor>& y,
+                                                  double slope) {
+  NhwcView yv{};
+  const NhwcView dv = check_grad_args(dy, s_out, y, &yv);
+  c10::cuda::CUDAGuard guard(dy.device());
+  const int pitch8 = (dv.C + 15) / 16 * 16;
+  at::Tensor full = empty_nhwc(dv.N, pitch8, dv.H, dv.W, dy.options().dtype(at::kFloat8_e5m2));
+  const long pixels = static_cast<long>(dv.N) * dv.H * dv.W;
+  at::Tensor src;
+  long src_pitch = 0;
+  at::Tensor partial = grad_amax(dy, dv, y, yv, slope, &src, &src_pitch);
+  cast_fp8_nhwc_kernel<E5M2><<<grid_for(pixels * (pitch8 / 16), kQuantThreads), kQuantThreads, 0,
+                               at::cuda::getCurrentCUDAStream()>>>(
       reinterpret_cast<const __nv_bfloat16*>(src.data_ptr()), pixels, dv.C, src_pitch, pitch8, partial.data_ptr<float>(),
-      blocks, reinterpret_cast<uint8_t*>(full.data_ptr()), s_out.data_ptr<float>());
+      static_cast<int>(partial.numel()), reinterpret_cast<uint8_t*>(full.data_ptr()), s_out.data_ptr<float>());
   C10_CUDA_KERNEL_LAUNCH_CHECK();
   return {full.narrow(1, 0, dv.C), src};
 }
@@ -305,4 +440,7 @@ TORCH_LIBRARY_FRAGMENT(poseidon, m) {
   m.def("fp8_quant_weight(Tensor w, int cgk, Tensor(a!) s_w_out) -> Tensor", &psd::fp8_quant_weight);
   m.def("fp8_quant_grad(Tensor dy, Tensor(a!) s_out, Tensor? y, float slope) -> (Tensor, Tensor)", &psd::fp8_quant_grad);
   m.def("fp8_quant_weight_dgrad(Tensor w, int groups, int cok, Tensor(a!) s_out) -> Tensor", &psd::fp8_quant_weight_dgrad);
+  m.def("fp8_quant_act_t(Tensor x, Tensor(a!) s_out) -> Tensor", &psd::fp8_quant_act_t);
+  m.def("fp8_quant_grad_t(Tensor dy, Tensor(a!) s_out, Tensor? y, float slope, bool nhwc) -> (Tensor, Tensor, Tensor)",
+        &psd::fp8_quant_grad_t);
 }

@@ -48,7 +48,7 @@ class NetContext:
         self.data_shape_hint = data_shape_hint
         self.model_dir = model_dir
         self.channels_last = channels_last
-        self.fp8 = fp8                  # sm100 engine: "off" | "fprop" | "fprop+dgrad" fp8 convolutions (None: POSEIDON_FP8)
+        self.fp8 = fp8                  # sm100 engine: an ops/sm100.py FP8_MODES value (None: POSEIDON_FP8)
 
     @property
     def train(self):

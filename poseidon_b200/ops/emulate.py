@@ -68,6 +68,13 @@ def e5m2_quant(v: torch.Tensor, s) -> torch.Tensor:
     return torch.clamp(v.float() * s, -E5M2_MAX, E5M2_MAX).to(E5M2)
 
 
+def chwn_images(n: int) -> int:
+    """Images per channel row of the fp8 weight gradient's batch-innermost copies: 16, 32, 64 or a multiple of 128."""
+    if n <= 64:
+        return 16 if n <= 16 else (32 if n <= 32 else 64)
+    return (n + 127) // 128 * 128
+
+
 def e4m3_quant(v: torch.Tensor, s) -> torch.Tensor:
     """e4m3(v · s) as cvt.rn.satfinite does it: clamp to ±448 first (torch's cast gives NaN above 464), NaN stays NaN."""
     return torch.clamp(v.float() * s, -E4M3_MAX, E4M3_MAX).to(E4M3)
@@ -302,6 +309,40 @@ class EmulatedKernels:
         out = torch.zeros((groups * cg, r * s_, cok), dtype=E4M3)
         out[..., :cout_g].copy_(e4m3_quant(rows, s.view(-1, 1, 1)))
         return out.reshape(groups * cg, r * s_ * cok)
+
+    # ------------------------------------------------------------------------------------------ fp8 weight gradient
+    @staticmethod
+    def _chwn(q: torch.Tensor) -> torch.Tensor:
+        """[N, C, H, W] fp8 -> the batch-innermost copy [C, H, W, Np], Np = N rounded up to 16, 32, 64 or a multiple of 128,
+        pad images zero."""
+        n, c, h, w = q.shape
+        out = torch.zeros((c, h, w, chwn_images(n)), dtype=q.dtype)
+        out[..., :n].copy_(q.permute(1, 2, 3, 0))
+        return out
+
+    def fp8_quant_act_t(self, x, s_out):
+        """bf16 NHWC (pitch may exceed C) -> e4m3 [C, H, W, Np], the transpose of fp8_quant_act's result;
+        s_out <- 1 / s (csrc/ops/fp8_quant.cu fp8_quant_act_t)."""
+        return self._chwn(self.fp8_quant_act(x, s_out))
+
+    def fp8_quant_grad_t(self, dy, s_out, y, slope, nhwc):
+        """(e5m2 [C, OH, OW, Np], fp8_quant_grad's NHWC copy when nhwc else an empty tensor, the bf16 dY that was
+        cast) (csrc/ops/fp8_quant.cu fp8_quant_grad_t)."""
+        q, src = self.fp8_quant_grad(dy, s_out, y, slope)
+        return self._chwn(q), q if nhwc else torch.empty(0, dtype=E5M2), src
+
+    def conv_wgrad_fp8(self, dy8t, x8t, s_dy, s_x, dw, kernel, pad, groups, alpha, cgk):
+        """dw[Cout, R*S*Cg] fp32 += alpha · s_dy · s_x · (stride-1 weight gradient of the fp8 copies)
+        (csrc/gemm/conv_ops.cu conv_wgrad_fp8)."""
+        r, s = kernel
+        assert dy8t.shape[3] == x8t.shape[3] == chwn_images(dy8t.shape[3]) and cgk >= x8t.shape[0] // groups and cgk % 64 == 0
+        assert tuple(dy8t.shape[1:3]) == (x8t.shape[1] + 2 * pad[0] - r + 1, x8t.shape[2] + 2 * pad[1] - s + 1)
+        x = x8t.float().permute(3, 0, 1, 2)
+        d = dy8t.float().permute(3, 0, 1, 2)
+        cout, cg = d.shape[1], x.shape[1] // groups
+        g = torch.nn.grad.conv2d_weight(x, (cout, cg, r, s), d, 1, tuple(pad), 1, groups)
+        g = g.permute(0, 2, 3, 1).reshape(cout, r * s * cg)
+        dw.add_(g * (s_dy.float().reshape(()) * s_x.float().reshape(())), alpha=alpha)
 
     def conv_dgrad_fp8(self, dy8, wt8, s_dy, s_wt, kernel, pad, groups, H, W, mask, slope):
         """Stride-1 data gradient conv_transpose(dy8, wt8) · s_dy · s_wt[ci], producer-ReLU mask in the epilogue

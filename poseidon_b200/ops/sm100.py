@@ -111,14 +111,16 @@ def _pad64(c: int) -> int:
     return p if (p - c) * 100 <= 34 * c else c
 
 
-FP8_MODES = ("off", "fprop", "fprop+dgrad")
+FP8_MODES = ("off", "fprop", "fprop+dgrad", "fprop+dgrad+wgrad")
 
 
 def resolve_fp8(mode: Optional[str] = None) -> str:
     """The engine's fp8 setting: ``mode`` when given, else ``POSEIDON_FP8`` (unset: "off").
     "fprop": eligible convolutions run their forward pass on e4m3 operands (data / weight gradients stay bf16).
     "fprop+dgrad": as "fprop", and eligible stride-1 convolutions also compute their data gradient from e5m2 dY and e4m3
-    weights (weight / bias gradients stay bf16 / fp32)."""
+    weights (weight / bias gradients stay bf16 / fp32).
+    "fprop+dgrad+wgrad": as "fprop+dgrad", and eligible stride-1 convolutions also compute their weight gradient from
+    e5m2 dY and e4m3 X (bias gradients stay fp32 from the bf16 dY)."""
     m = str(mode if mode is not None else os.environ.get("POSEIDON_FP8", "off")).lower()
     if m not in FP8_MODES:
         raise ValueError(f"fp8 must be one of {', '.join(FP8_MODES)}, got '{m}'")
@@ -202,7 +204,7 @@ class ConvState:
         # per tap (Cg rounded up to 128: one 128-byte K block); decided once here
         mode = resolve_fp8(fp8)
         self.fp8, self.fp8_reason = False, "fp8 off"
-        if mode in ("fprop", "fprop+dgrad"):
+        if mode != "off":
             self.fp8, self.fp8_reason = self._fp8_eligible(layer)
         self.cgk8 = _round128(self.cg) if self.fp8 else 0
         self.s_x: Optional[torch.Tensor] = None       # fp8 dequantisation scales, written by the quantisers every forward
@@ -210,11 +212,18 @@ class ConvState:
         # fp8 data gradient (opt-in, decided independently of the forward): e5m2 dY x e4m3 weights quantised on every
         # backward from dY and the fp32 master, Cok8 slots per tap (Cout_g rounded up to 128)
         self.fp8_dgrad, self.fp8_dgrad_reason = False, "fp8 dgrad off"
-        if mode == "fprop+dgrad":
+        if mode in ("fprop+dgrad", "fprop+dgrad+wgrad"):
             self.fp8_dgrad, self.fp8_dgrad_reason = self._fp8_dgrad_eligible(layer)
         self.cok8 = _round128(self.Cout // self.groups) if self.fp8_dgrad else 0
         self.s_dy: Optional[torch.Tensor] = None      # written by the quantisers every backward
         self.s_wt: Optional[torch.Tensor] = None
+        # fp8 weight gradient (opt-in, decided independently of the other two): e5m2 dY x e4m3 X in batch-innermost copies
+        # quantised on every backward, Cgkw8 column slots per tap (Cg rounded up to 64: one B box per 64 columns)
+        self.fp8_wgrad, self.fp8_wgrad_reason = False, "fp8 wgrad off"
+        if mode == "fprop+dgrad+wgrad":
+            self.fp8_wgrad, self.fp8_wgrad_reason = self._fp8_wgrad_eligible(layer)
+        self.cgkw8 = _pad64(self.cg) if self.fp8_wgrad else 0
+        self.s_xw: Optional[torch.Tensor] = None      # X's scale for the weight gradient (not the forward's s_x)
         self.wbp: Optional[torch.Tensor] = None      # channel-padded copy of wb (derived, refreshed when wb changes)
         self.dirty_wbp = True
         self.wb: Optional[torch.Tensor] = None
@@ -300,6 +309,26 @@ class ConvState:
         if (p - cout_g) * 100 > 34 * cout_g:
             return False, f"Cout_g {cout_g} -> {p} slots wastes more than a third"
         return True, f"Cout_g {cout_g} -> {p} slots"
+
+    def _fp8_wgrad_eligible(self, layer):
+        """(fp8 weight gradient?, reason): a stride-1 TAP-mode layer with channel counts in multiples of 8 whose Cg is a
+        multiple of 64 or rounds up to one wasting at most a third (_pad64): every 64-column chunk of the reduction's
+        X side is one tap.  Batch only sets the k-block layout, so it does not enter the rule."""
+        if self.row_mode or self.s2d or self.pad8:
+            return False, "first-layer layout (ROW / s2d / 8-channel pad)"
+        if tuple(layer.stride) != (1, 1):
+            return False, "strided"
+        cout_g = self.Cout // self.groups
+        if self.Coutp != self.Cout or self.cg % 8 or cout_g % 8:
+            return False, "channel counts are not multiples of 8"
+        if self.R > 15 or self.S > 15:
+            return False, "kernel larger than 15"
+        if any(p >= k for p, k in zip(layer.pad, (self.R, self.S))):
+            return False, "padding not below the kernel extent"
+        p = _pad64(self.cg)
+        if p % 64:
+            return False, f"Cg {self.cg} does not round up to a multiple of 64 within a third"
+        return True, f"Cg {self.cg} -> {p} columns per tap"
 
     # physical [Cout, Kw] fp32 view of the master weight (TAP mode only)
     def w2d(self) -> torch.Tensor:
@@ -488,7 +517,12 @@ class _ConvFn(torch.autograd.Function):
             dy = dyp
         else:
             dy = as_kernel_input(dy)
-            if st.fp8_dgrad and ctx.needs_input_grad[0]:
+            if st.fp8_wgrad and ctx.needs_input_grad[1]:
+                # e5m2 dY for the weight gradient (batch-innermost copy, plus the NHWC copy of an fp8 data gradient):
+                # one amax pass (ReLU backward fused in as below) and one cast pass, on this stream before the fork
+                dy8t, dy8, dy = _fp8_quant_grad_t(k, st, dy, y if not st.consumer_masks else None, ctx.relu_slope,
+                                                  st.fp8_dgrad and ctx.needs_input_grad[0])
+            elif st.fp8_dgrad and ctx.needs_input_grad[0]:
                 # e5m2 dY: amax pass (with this layer's ReLU backward fused in when it masks its own gradient; the
                 # weight / bias gradients below then read the masked bf16 dY it writes) and cast
                 dy8, dy = _fp8_quant_grad(k, st, dy, y if not st.consumer_masks else None, ctx.relu_slope)
@@ -538,11 +572,18 @@ class _ConvFn(torch.autograd.Function):
             side.wait_event(fork)
             dy.record_stream(side)
             xin.record_stream(side)
+            if st.fp8_wgrad and dw2 is not None:
+                dy8t.record_stream(side)
             torch.cuda.set_stream(side)
         try:
             if dw2 is not None:
                 if st.s2d:
                     k.conv_wgrad(xin, dy, dw2, [st.Rq, st.Sq], [1, 1], [0, 0], 1, 0, 1.0, 0)
+                elif st.fp8_wgrad:
+                    # e4m3 X (its own scale) and the fp8 GEMM, on the weight-gradient side stream
+                    x8t = k.fp8_quant_act_t(xin, st.s_xw)
+                    k.conv_wgrad_fp8(dy8t, x8t, st.s_dy, st.s_xw, dw2, [st.R, st.S], list(ctx.conv_pad), st.groups, 1.0,
+                                     st.cgkw8)
                 else:
                     k.conv_wgrad(xin, dy, dw2, [st.R, st.S], list(stride), list(ctx.conv_pad), st.groups,
                                  1 if (st.row_mode and not st.pad8) else 0, 1.0, st.cgk if not st.row_mode else 0)
@@ -608,6 +649,18 @@ def _fp8_quant_grad(k, st: ConvState, dy, y, slope):
         st.s_dy = torch.ones(1, device=dy.device, dtype=torch.float32)
         st.s_wt = torch.ones(st.Cp, device=dy.device, dtype=torch.float32)
     return k.fp8_quant_grad(dy, st.s_dy, y, float(slope or 0.0))
+
+
+def _fp8_quant_grad_t(k, st: ConvState, dy, y, slope, nhwc: bool):
+    """e5m2 dY for the fp8 weight gradient: returns (dy8t, dy8 for an fp8 data gradient (nhwc) else None, the bf16 dY the
+    bias gradient reads), with the scale and mask of _fp8_quant_grad."""
+    if st.s_dy is None:
+        st.s_dy = torch.ones(1, device=dy.device, dtype=torch.float32)
+        st.s_wt = torch.ones(st.Cp, device=dy.device, dtype=torch.float32)
+    if st.s_xw is None:
+        st.s_xw = torch.ones(1, device=dy.device, dtype=torch.float32)
+    dy8t, dy8, src = k.fp8_quant_grad_t(dy, st.s_dy, y, float(slope or 0.0), nhwc)
+    return dy8t, (dy8 if nhwc else None), src
 
 
 _DGRAD_PACK = os.environ.get("POSEIDON_DGRAD_PACK", "0") == "1"      # A/B switch: always use the packed dgrad operand

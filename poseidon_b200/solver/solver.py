@@ -110,7 +110,7 @@ class Solver:
         self.rank_ctx = rank_ctx
         self.engine = engine
         from ..ops.sm100 import fp8_for_engine
-        self.fp8 = fp8_for_engine(engine, fp8)     # "fprop" / "fprop+dgrad": fp8 convolutions (ops/sm100.py)
+        self.fp8 = fp8_for_engine(engine, fp8)     # "fprop" / "fprop+dgrad" / "fprop+dgrad+wgrad" (ops/sm100.py)
         self.staleness = int(staleness)
         self.aggr_fraction = float(aggr_fraction)
         # gradients on the network as bf16 (the reference's DenseFloat16 row oplogs: fp16 on the wire, fp32 at rest);
