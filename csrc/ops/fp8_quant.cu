@@ -14,6 +14,9 @@
 //                      dY (e5m2), Np = N rounded up to 16, 32, 64 or a multiple of 128 (a 128-byte row then holds whole
 //                      columns or whole image chunks), pad images zero; scale rules, mask and kernels as fp8_quant_act /
 //                      fp8_quant_grad.
+//   fp8_quant_act_delayed / fp8_quant_act_t_delayed / fp8_quant_grad_delayed / fp8_quant_grad_t_delayed : the same
+//                      results with delayed scaling (an amax history in device memory, one pass; see "Delayed scaling"
+//                      below); fp8_quant_act_t_delayed can also write the NHWC copy, so one pass gives x8 and x8t.
 //
 // Scaling is just in time: s = MAX / amax(|v|) (MAX = 448 for e4m3, 57344 for e5m2; 1 when amax == 0),
 // q = cvt.rn.satfinite(v * s), and 1 / s is stored for the GEMM epilogue.  amax uses fmaxf, which skips NaN, so a NaN
@@ -433,6 +436,307 @@ at::Tensor fp8_quant_weight_dgrad(const at::Tensor& w, int64_t groups, int64_t c
   return w8;
 }
 
+// ---------------------------------------------------------------------------------------------------------------------
+// Delayed scaling (fp8_scaling="delayed"): the scale comes from an amax history in device memory instead of an amax pass,
+// so each quantiser below is one launch that reads its input once.
+//
+// ring: int32 [kRingWords] per scaled tensor.  Words [0, 16) are the history (fp32 amax bit patterns, all >= 0), then the
+// position (the slot this call records into), a CTA ticket and the running amax of the call in flight (the last two are
+// zero between calls).  One call:
+//   * scales with s = quant_scale(max of the 15 other slots); a seeding call (`seed`: the ring's first) runs the amax pass
+//     first and scales with that amax instead, so its results are the just-in-time quantiser's bit for bit;
+//   * casts with cvt.rn.satfinite (values beyond the window's amax saturate to +-MAX); an infinite element becomes NaN, as
+//     the just-in-time scale (0 when the amax is infinite) makes it, and NaN stays NaN;
+//   * stores 1 / s in s_out for the GEMM epilogue;
+//   * records the tensor's own amax (fmaxf: NaN skipped, +Inf kept) with an integer atomicMax on the bit patterns: max
+//     does not depend on order, so the bits repeat from run to run.  The CTA that finishes last writes it into the slot
+//     (every slot when seeding), clears the scratch words and advances the position.  Each CTA reads the position before
+//     it takes its ticket, and the slot being recorded is outside the window, so every CTA of a launch uses one scale.
+constexpr int kAmaxHistory = 16;
+constexpr int kRingPos = kAmaxHistory, kRingTicket = kAmaxHistory + 1, kRingAmax = kAmaxHistory + 2;
+constexpr int kRingWords = kAmaxHistory + 3;
+
+struct DelayedRing {
+  int* ring;
+  const float* partial;        // seeding call: the amax pass's partial maxima (nullptr: scale from the history)
+  int nparts;
+};
+
+// Every thread of every CTA: the launch's scale; *pos: the slot the launch records into.
+template <typename F>
+__device__ __forceinline__ float delayed_scale(const DelayedRing& r, float* red, int* pos) {
+  *pos = r.ring[kRingPos];
+  float m = 0.f;
+  if (r.partial != nullptr) {
+    for (int i = threadIdx.x; i < r.nparts; i += blockDim.x) m = fmaxf(m, r.partial[i]);
+    m = block_max(m, red);
+  } else {
+#pragma unroll
+    for (int i = 0; i < kAmaxHistory; ++i)
+      if (i != *pos) m = fmaxf(m, __int_as_float(r.ring[i]));
+  }
+  return quant_scale<F>(m);
+}
+
+// Every thread, after its last element (m: its amax of |v|): the CTA's amax joins the launch's; the last CTA records it.
+__device__ __forceinline__ void delayed_record(const DelayedRing& r, float m, float* red, int pos) {
+  m = block_max(m, red);
+  if (threadIdx.x != 0) return;
+  int* ring = r.ring;
+  atomicMax(ring + kRingAmax, __float_as_int(m));
+  __threadfence();
+  const unsigned ctas = gridDim.x * gridDim.y * gridDim.z;
+  if (atomicAdd(reinterpret_cast<unsigned*>(ring + kRingTicket), 1u) != ctas - 1) return;
+  __threadfence();
+  const int a = atomicExch(ring + kRingAmax, 0);
+  if (r.partial != nullptr) {
+#pragma unroll
+    for (int i = 0; i < kAmaxHistory; ++i) ring[i] = a;
+  } else {
+    ring[pos] = a;
+  }
+  ring[kRingTicket] = 0;
+  ring[kRingPos] = (pos + 1) % kAmaxHistory;
+}
+
+// v * s for the delayed casts: an infinite element becomes NaN (see above)
+__device__ __forceinline__ float scaled(float v, float s) { return isinf(v) ? __int_as_float(0x7fffffff) : v * s; }
+
+// 8 channels of x at pixel px from channel c; kMask: dY masked by the layer's own ReLU backward (mask_amax_nhwc_kernel's
+// formula, so relu_bwd's bits), also written dense (pixel pitch C) into `masked`, and returned as the bf16 values stored.
+template <bool kMask>
+__device__ __forceinline__ void load8(const __nv_bfloat16* x, long pitch, const __nv_bfloat16* y, long pitch_y, float slope,
+                                      __nv_bfloat16* masked, int C, long px, int c, float (&f)[8]) {
+  unpack8(ld8(x + px * pitch + c), f);
+  if constexpr (kMask) {
+    float g[8];
+    unpack8(ld8(y + px * pitch_y + c), g);
+#pragma unroll
+    for (int k = 0; k < 8; ++k) f[k] = g[k] > 0.f ? f[k] : f[k] * slope;
+    const bf16x8 q = pack8(f);
+    st8(masked + px * C + c, q);
+    unpack8(q, f);
+  }
+}
+
+// The delayed cast_fp8_nhwc_kernel (same output layout), with the dY mask of mask_amax_nhwc_kernel fused in (kMask).
+template <typename F, bool kMask>
+__global__ void __launch_bounds__(kQuantThreads) cast_fp8_nhwc_delayed_kernel(
+    const __nv_bfloat16* __restrict__ x, long pitch, const __nv_bfloat16* __restrict__ y, long pitch_y, float slope,
+    __nv_bfloat16* __restrict__ masked, long pixels, int C, int pitch8, DelayedRing ring, uint8_t* __restrict__ q8,
+    float* __restrict__ s_out) {
+  __shared__ float red[kQuantThreads / 32];
+  int pos;
+  const float s = delayed_scale<F>(ring, red, &pos);
+  if (blockIdx.x == 0 && threadIdx.x == 0) *s_out = 1.f / s;
+  const int cpp = pitch8 / 16;
+  const long items = pixels * cpp;
+  float m = 0.f;
+  for (long i = blockIdx.x * static_cast<long>(blockDim.x) + threadIdx.x; i < items; i += static_cast<long>(gridDim.x) * blockDim.x) {
+    const long px = i / cpp;
+    const int c0 = static_cast<int>(i - px * cpp) * 16;
+    float a[8], b[8];
+    load8<kMask>(x, pitch, y, pitch_y, slope, masked, C, px, c0, a);
+    if (c0 + 8 < C) {
+      load8<kMask>(x, pitch, y, pitch_y, slope, masked, C, px, c0 + 8, b);
+    } else {
+#pragma unroll
+      for (int k = 0; k < 8; ++k) b[k] = 0.f;
+    }
+#pragma unroll
+    for (int k = 0; k < 8; ++k) m = fmaxf(m, fmaxf(fabsf(a[k]), fabsf(b[k])));
+    uint4 q;
+    q.x = cvt_fp8x2<F>(scaled(a[0], s), scaled(a[1], s)) | (cvt_fp8x2<F>(scaled(a[2], s), scaled(a[3], s)) << 16);
+    q.y = cvt_fp8x2<F>(scaled(a[4], s), scaled(a[5], s)) | (cvt_fp8x2<F>(scaled(a[6], s), scaled(a[7], s)) << 16);
+    q.z = cvt_fp8x2<F>(scaled(b[0], s), scaled(b[1], s)) | (cvt_fp8x2<F>(scaled(b[2], s), scaled(b[3], s)) << 16);
+    q.w = cvt_fp8x2<F>(scaled(b[4], s), scaled(b[5], s)) | (cvt_fp8x2<F>(scaled(b[6], s), scaled(b[7], s)) << 16);
+    *reinterpret_cast<uint4*>(q8 + px * pitch8 + c0) = q;
+  }
+  delayed_record(ring, m, red, pos);
+}
+
+// The delayed cast_fp8_chwn_kernel (same tiles and outputs: yt, and the NHWC copy when y8 != nullptr), with the dY mask
+// fused in (kMask).
+template <typename F, bool kMask>
+__global__ void __launch_bounds__(kQuantThreads) cast_fp8_chwn_delayed_kernel(
+    const __nv_bfloat16* __restrict__ x, int N, int Np, int C, int HW, long pitch, const __nv_bfloat16* __restrict__ y,
+    long pitch_y, float slope, __nv_bfloat16* __restrict__ masked, DelayedRing ring, uint8_t* __restrict__ yt,
+    uint8_t* __restrict__ y8, int pitch8, float* __restrict__ s_out) {
+  __shared__ float red[kQuantThreads / 32];
+  __shared__ __align__(16) uint8_t tile[kTileC][kTileN];
+  int pos;
+  const float s = delayed_scale<F>(ring, red, &pos);
+  if (blockIdx.x == 0 && blockIdx.y == 0 && blockIdx.z == 0 && threadIdx.x == 0) *s_out = 1.f / s;
+  const int hw = blockIdx.x, c0 = blockIdx.y * kTileC, n0 = blockIdx.z * kTileN;
+  float m = 0.f;
+  {
+    const int n = threadIdx.x / 8, v = threadIdx.x % 8;          // image n0 + n, channels c0 + 8v ..
+    const int nn = n0 + n, c = c0 + 8 * v;
+    uint32_t lo = 0, hi = 0;
+    if (nn < N && c < C) {
+      float a[8];
+      load8<kMask>(x, pitch, y, pitch_y, slope, masked, C, static_cast<long>(nn) * HW + hw, c, a);
+#pragma unroll
+      for (int k = 0; k < 8; ++k) m = fmaxf(m, fabsf(a[k]));
+      lo = cvt_fp8x2<F>(scaled(a[0], s), scaled(a[1], s)) | (cvt_fp8x2<F>(scaled(a[2], s), scaled(a[3], s)) << 16);
+      hi = cvt_fp8x2<F>(scaled(a[4], s), scaled(a[5], s)) | (cvt_fp8x2<F>(scaled(a[6], s), scaled(a[7], s)) << 16);
+    }
+    if (y8 != nullptr && nn < N && c < pitch8)
+      *reinterpret_cast<uint2*>(y8 + (static_cast<long>(nn) * HW + hw) * pitch8 + c) = make_uint2(lo, hi);
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      tile[8 * v + k][n] = static_cast<uint8_t>(lo >> (8 * k));
+      tile[8 * v + 4 + k][n] = static_cast<uint8_t>(hi >> (8 * k));
+    }
+  }
+  __syncthreads();
+  const int c = threadIdx.x / 4, n8 = (threadIdx.x % 4) * 8;
+  if (c0 + c < C && n0 + n8 < Np)
+    *reinterpret_cast<uint2*>(yt + (static_cast<long>(c0 + c) * HW + hw) * Np + n0 + n8) =
+        *reinterpret_cast<const uint2*>(&tile[c][n8]);
+  delayed_record(ring, m, red, pos);
+}
+
+static void check_ring(const at::Tensor& ring, const at::Tensor& x, const char* op) {
+  TORCH_CHECK(ring.is_cuda() && ring.device() == x.device() && ring.scalar_type() == at::kInt &&
+              ring.numel() == kRingWords && ring.is_contiguous(),
+              op, ": ring must be ", kRingWords, " contiguous int32 elements on the input's device");
+}
+
+// Source of a delayed launch: x itself, or (seeding) the amax pass's result.  With y (dY masked by the layer's own ReLU),
+// a seeding call masks in grad_amax and casts its dense copy; a steady-state call masks in the cast kernel itself.
+struct DelayedSrc {
+  at::Tensor src, partial;     // the bf16 tensor the cast reads (or writes, when it masks), the seed's partial maxima
+  long pitch;
+  bool mask;                   // the cast kernel applies the mask
+};
+
+static DelayedSrc delayed_src(const at::Tensor& x, const NhwcView& xv, const c10::optional<at::Tensor>& y,
+                              const NhwcView& yv, double slope, bool seed) {
+  DelayedSrc d{x, at::Tensor(), xv.pitch, false};
+  if (seed) {
+    d.partial = grad_amax(x, xv, y, yv, slope, &d.src, &d.pitch);
+  } else if (y.has_value()) {
+    d.src = empty_nhwc(xv.N, xv.C, xv.H, xv.W, x.options());
+    d.mask = true;
+  }
+  return d;
+}
+
+template <typename F>
+static void launch_nhwc_delayed(const at::Tensor& x, const NhwcView& xv, const DelayedSrc& d,
+                                const c10::optional<at::Tensor>& y, const NhwcView& yv, double slope, at::Tensor& ring,
+                                at::Tensor& q8, int pitch8, at::Tensor& s_out) {
+  const long pixels = static_cast<long>(xv.N) * xv.H * xv.W;
+  const DelayedRing r{ring.data_ptr<int>(), d.partial.defined() ? d.partial.data_ptr<float>() : nullptr,
+                      d.partial.defined() ? static_cast<int>(d.partial.numel()) : 0};
+  const int blocks = grid_for(pixels * (pitch8 / 16), kQuantThreads);
+  auto stream = at::cuda::getCurrentCUDAStream();
+  auto* q = reinterpret_cast<uint8_t*>(q8.data_ptr());
+  auto* out = reinterpret_cast<__nv_bfloat16*>(d.src.data_ptr());
+  if (d.mask)
+    cast_fp8_nhwc_delayed_kernel<F, true><<<blocks, kQuantThreads, 0, stream>>>(
+        reinterpret_cast<const __nv_bfloat16*>(x.data_ptr()), xv.pitch, reinterpret_cast<const __nv_bfloat16*>(y->data_ptr()),
+        yv.pitch, static_cast<float>(slope), out, pixels, xv.C, pitch8, r, q, s_out.data_ptr<float>());
+  else
+    cast_fp8_nhwc_delayed_kernel<F, false><<<blocks, kQuantThreads, 0, stream>>>(
+        out, d.pitch, nullptr, 0, 0.f, nullptr, pixels, xv.C, pitch8, r, q, s_out.data_ptr<float>());
+  C10_CUDA_KERNEL_LAUNCH_CHECK();
+}
+
+template <typename F>
+static void launch_chwn_delayed(const at::Tensor& x, const NhwcView& xv, const DelayedSrc& d,
+                                const c10::optional<at::Tensor>& y, const NhwcView& yv, double slope, at::Tensor& ring,
+                                int Np, at::Tensor& yt, at::Tensor* y8, int pitch8, at::Tensor& s_out) {
+  const dim3 grid(static_cast<unsigned>(xv.H * xv.W), static_cast<unsigned>((xv.C + kTileC - 1) / kTileC),
+                  static_cast<unsigned>((Np + kTileN - 1) / kTileN));
+  const DelayedRing r{ring.data_ptr<int>(), d.partial.defined() ? d.partial.data_ptr<float>() : nullptr,
+                      d.partial.defined() ? static_cast<int>(d.partial.numel()) : 0};
+  auto stream = at::cuda::getCurrentCUDAStream();
+  auto* t = reinterpret_cast<uint8_t*>(yt.data_ptr());
+  uint8_t* q = y8 != nullptr ? reinterpret_cast<uint8_t*>(y8->data_ptr()) : nullptr;
+  auto* out = reinterpret_cast<__nv_bfloat16*>(d.src.data_ptr());
+  if (d.mask)
+    cast_fp8_chwn_delayed_kernel<F, true><<<grid, kQuantThreads, 0, stream>>>(
+        reinterpret_cast<const __nv_bfloat16*>(x.data_ptr()), xv.N, Np, xv.C, xv.H * xv.W, xv.pitch,
+        reinterpret_cast<const __nv_bfloat16*>(y->data_ptr()), yv.pitch, static_cast<float>(slope), out, r, t, q, pitch8,
+        s_out.data_ptr<float>());
+  else
+    cast_fp8_chwn_delayed_kernel<F, false><<<grid, kQuantThreads, 0, stream>>>(
+        out, xv.N, Np, xv.C, xv.H * xv.W, d.pitch, nullptr, 0, 0.f, nullptr, r, t, q, pitch8, s_out.data_ptr<float>());
+  C10_CUDA_KERNEL_LAUNCH_CHECK();
+}
+
+static NhwcView check_act_args(const at::Tensor& x, const at::Tensor& s_out, const at::Tensor& ring, const char* op) {
+  TORCH_CHECK(x.is_cuda() && x.scalar_type() == at::kBFloat16, op, ": bf16 CUDA input expected");
+  TORCH_CHECK(s_out.is_cuda() && s_out.scalar_type() == at::kFloat && s_out.numel() == 1 && s_out.is_contiguous(),
+              op, ": s_out must be one fp32 element");
+  check_ring(ring, x, op);
+  const NhwcView xv = nhwc_view(x);
+  TORCH_CHECK(xv.C % 8 == 0 && xv.pitch % 8 == 0 && (reinterpret_cast<uintptr_t>(x.data_ptr()) & 15) == 0,
+              op, ": channels and pixel pitch must be multiples of 8 (16-byte vectors)");
+  return xv;
+}
+
+// fp8_quant_act with delayed scaling: same input rules and result; ring: the input's history; seed: the ring's first call.
+at::Tensor fp8_quant_act_delayed(const at::Tensor& x, at::Tensor s_out, at::Tensor ring, bool seed) {
+  const NhwcView xv = check_act_args(x, s_out, ring, "fp8_quant_act_delayed");
+  c10::cuda::CUDAGuard guard(x.device());
+  const int pitch8 = (xv.C + 15) / 16 * 16;
+  at::Tensor full = empty_nhwc(xv.N, pitch8, xv.H, xv.W, x.options().dtype(at::kFloat8_e4m3fn));
+  const DelayedSrc d = delayed_src(x, xv, c10::nullopt, xv, 0.0, seed);
+  launch_nhwc_delayed<E4M3>(x, xv, d, c10::nullopt, xv, 0.0, ring, full, pitch8, s_out);
+  return full.narrow(1, 0, xv.C);
+}
+
+// fp8_quant_act_t with delayed scaling, returning (the batch-innermost e4m3 copy, with nhwc also fp8_quant_act's NHWC copy
+// else an empty tensor): one read of x gives the forward's x8 and the weight gradient's x8t with the same scale.
+std::tuple<at::Tensor, at::Tensor> fp8_quant_act_t_delayed(const at::Tensor& x, at::Tensor s_out, at::Tensor ring, bool seed,
+                                                           bool nhwc) {
+  const NhwcView xv = check_act_args(x, s_out, ring, "fp8_quant_act_t_delayed");
+  TORCH_CHECK(static_cast<long>(xv.H) * xv.W < (1L << 31), "fp8_quant_act_t_delayed: too many pixels per image");
+  c10::cuda::CUDAGuard guard(x.device());
+  const int Np = chwn_images(xv.N), pitch8 = (xv.C + 15) / 16 * 16;
+  at::Tensor xt = at::empty({xv.C, xv.H, xv.W, Np}, x.options().dtype(at::kFloat8_e4m3fn));
+  at::Tensor full = nhwc ? empty_nhwc(xv.N, pitch8, xv.H, xv.W, x.options().dtype(at::kFloat8_e4m3fn))
+                         : at::empty({0}, x.options().dtype(at::kFloat8_e4m3fn));
+  const DelayedSrc d = delayed_src(x, xv, c10::nullopt, xv, 0.0, seed);
+  launch_chwn_delayed<E4M3>(x, xv, d, c10::nullopt, xv, 0.0, ring, Np, xt, nhwc ? &full : nullptr, pitch8, s_out);
+  return {xt, nhwc ? full.narrow(1, 0, xv.C) : full};
+}
+
+// fp8_quant_grad with delayed scaling: same arguments, mask and results, plus the dY history and the seed flag.
+std::tuple<at::Tensor, at::Tensor> fp8_quant_grad_delayed(const at::Tensor& dy, at::Tensor s_out, at::Tensor ring, bool seed,
+                                                          const c10::optional<at::Tensor>& y, double slope) {
+  NhwcView yv{};
+  const NhwcView dv = check_grad_args(dy, s_out, y, &yv);
+  check_ring(ring, dy, "fp8_quant_grad_delayed");
+  c10::cuda::CUDAGuard guard(dy.device());
+  const int pitch8 = (dv.C + 15) / 16 * 16;
+  at::Tensor full = empty_nhwc(dv.N, pitch8, dv.H, dv.W, dy.options().dtype(at::kFloat8_e5m2));
+  const DelayedSrc d = delayed_src(dy, dv, y, yv, slope, seed);
+  launch_nhwc_delayed<E5M2>(dy, dv, d, y, yv, slope, ring, full, pitch8, s_out);
+  return {full.narrow(1, 0, dv.C), d.src};
+}
+
+// fp8_quant_grad_t with delayed scaling: same arguments, mask and results, plus the dY history and the seed flag.
+std::tuple<at::Tensor, at::Tensor, at::Tensor> fp8_quant_grad_t_delayed(const at::Tensor& dy, at::Tensor s_out, at::Tensor ring,
+                                                                        bool seed, const c10::optional<at::Tensor>& y,
+                                                                        double slope, bool nhwc) {
+  NhwcView yv{};
+  const NhwcView dv = check_grad_args(dy, s_out, y, &yv);
+  check_ring(ring, dy, "fp8_quant_grad_t_delayed");
+  TORCH_CHECK(static_cast<long>(dv.H) * dv.W < (1L << 31), "fp8_quant_grad_t_delayed: too many pixels per image");
+  c10::cuda::CUDAGuard guard(dy.device());
+  const int Np = chwn_images(dv.N), pitch8 = (dv.C + 15) / 16 * 16;
+  at::Tensor dyt = at::empty({dv.C, dv.H, dv.W, Np}, dy.options().dtype(at::kFloat8_e5m2));
+  at::Tensor full = nhwc ? empty_nhwc(dv.N, pitch8, dv.H, dv.W, dy.options().dtype(at::kFloat8_e5m2))
+                         : at::empty({0}, dy.options().dtype(at::kFloat8_e5m2));
+  const DelayedSrc d = delayed_src(dy, dv, y, yv, slope, seed);
+  launch_chwn_delayed<E5M2>(dy, dv, d, y, yv, slope, ring, Np, dyt, nhwc ? &full : nullptr, pitch8, s_out);
+  return {dyt, nhwc ? full.narrow(1, 0, dv.C) : full, d.src};
+}
+
 }  // namespace psd
 
 TORCH_LIBRARY_FRAGMENT(poseidon, m) {
@@ -443,4 +747,12 @@ TORCH_LIBRARY_FRAGMENT(poseidon, m) {
   m.def("fp8_quant_act_t(Tensor x, Tensor(a!) s_out) -> Tensor", &psd::fp8_quant_act_t);
   m.def("fp8_quant_grad_t(Tensor dy, Tensor(a!) s_out, Tensor? y, float slope, bool nhwc) -> (Tensor, Tensor, Tensor)",
         &psd::fp8_quant_grad_t);
+  m.def("fp8_quant_act_delayed(Tensor x, Tensor(a!) s_out, Tensor(b!) ring, bool seed) -> Tensor",
+        &psd::fp8_quant_act_delayed);
+  m.def("fp8_quant_act_t_delayed(Tensor x, Tensor(a!) s_out, Tensor(b!) ring, bool seed, bool nhwc) -> (Tensor, Tensor)",
+        &psd::fp8_quant_act_t_delayed);
+  m.def("fp8_quant_grad_delayed(Tensor dy, Tensor(a!) s_out, Tensor(b!) ring, bool seed, Tensor? y, float slope) -> "
+        "(Tensor, Tensor)", &psd::fp8_quant_grad_delayed);
+  m.def("fp8_quant_grad_t_delayed(Tensor dy, Tensor(a!) s_out, Tensor(b!) ring, bool seed, Tensor? y, float slope, "
+        "bool nhwc) -> (Tensor, Tensor, Tensor)", &psd::fp8_quant_grad_t_delayed);
 }

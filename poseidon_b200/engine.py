@@ -40,7 +40,7 @@ class CaffeEngine:
     def __init__(self, solver_param, rank_ctx=None, *, engine: str = "auto", comm: str = "auto", svb: bool = True,
                  staleness: int = 0, grad_reduce: str = "sum", sfb_mode: str = "auto", model_dir: Optional[str] = None,
                  data_shape_hint=None, aggr_fraction: float = 0.1, wire_dtype: Optional[str] = None,
-                 fp8: Optional[str] = None):
+                 fp8: Optional[str] = None, fp8_scaling: Optional[str] = None):
         if isinstance(solver_param, str):
             model_dir = model_dir or os.path.dirname(os.path.abspath(solver_param))
             solver_param = P.read_solver(solver_param)
@@ -48,7 +48,7 @@ class CaffeEngine:
         self.rank_ctx = rank_ctx
         self.opts = dict(engine=engine, comm=comm, svb=svb, staleness=staleness, grad_reduce=grad_reduce,
                          sfb_mode=sfb_mode, model_dir=model_dir, data_shape_hint=data_shape_hint,
-                         aggr_fraction=aggr_fraction, wire_dtype=wire_dtype, fp8=fp8)
+                         aggr_fraction=aggr_fraction, wire_dtype=wire_dtype, fp8=fp8, fp8_scaling=fp8_scaling)
         self.solver = None
 
     # ---------------------------------------------------------------------------------- bring-up

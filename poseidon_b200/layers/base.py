@@ -37,7 +37,7 @@ class NetContext:
 
     def __init__(self, phase=P.TRAIN, device="cpu", engine="torch", dtype=torch.float32,
                  rank=0, world_size=1, seed=None, data_shape_hint=None, model_dir=None,
-                 channels_last=False, fp8=None):
+                 channels_last=False, fp8=None, fp8_scaling=None):
         self.phase = phase
         self.device = torch.device(device)
         self.engine = engine            # "torch" (cpu / vendor libs) | "sm100" (our kernels)
@@ -49,6 +49,7 @@ class NetContext:
         self.model_dir = model_dir
         self.channels_last = channels_last
         self.fp8 = fp8                  # sm100 engine: an ops/sm100.py FP8_MODES value (None: POSEIDON_FP8)
+        self.fp8_scaling = fp8_scaling  # an ops/sm100.py FP8_SCALINGS value (None: POSEIDON_FP8_SCALING when fp8 is on)
 
     @property
     def train(self):

@@ -29,22 +29,25 @@ def plan_sm100(net) -> None:
 
     # engine state (operand layouts) for every learnable layer
     fp8 = sm100.resolve_fp8(getattr(net.ctx, "fp8", None))
+    scaling = sm100.resolve_fp8_scaling(getattr(net.ctx, "fp8_scaling", None), fp8)
+    tail = "; scaling delayed" if scaling == "delayed" else ""
     for i, layer in enumerate(net.layers):
         if layer.type_name == "CONVOLUTION":
             cin = net.blob_shapes[net.bottom_names[i][0]][1]
             try:
-                st = sm100.conv_state(layer, cin, fp8)
+                st = sm100.conv_state(layer, cin, fp8, scaling)
             except ValueError as e:
                 raise ValueError(f"layer {net.layer_names[i]}: {e}") from e
             if fp8 == "fprop" and net.ctx.rank == 0:
-                log.info("sm100 plan: conv %s: %s (%s)", net.layer_names[i], "fp8" if st.fp8 else "bf16", st.fp8_reason)
+                log.info("sm100 plan: conv %s: %s (%s)%s", net.layer_names[i], "fp8" if st.fp8 else "bf16", st.fp8_reason,
+                         tail)
             elif fp8 == "fprop+dgrad" and net.ctx.rank == 0:
-                log.info("sm100 plan: conv %s: %s (%s); dgrad %s (%s)", net.layer_names[i], "fp8" if st.fp8 else "bf16",
-                         st.fp8_reason, "fp8" if st.fp8_dgrad else "bf16", st.fp8_dgrad_reason)
+                log.info("sm100 plan: conv %s: %s (%s); dgrad %s (%s)%s", net.layer_names[i], "fp8" if st.fp8 else "bf16",
+                         st.fp8_reason, "fp8" if st.fp8_dgrad else "bf16", st.fp8_dgrad_reason, tail)
             elif fp8 == "fprop+dgrad+wgrad" and net.ctx.rank == 0:
-                log.info("sm100 plan: conv %s: %s (%s); dgrad %s (%s); wgrad %s (%s)", net.layer_names[i],
+                log.info("sm100 plan: conv %s: %s (%s); dgrad %s (%s); wgrad %s (%s)%s", net.layer_names[i],
                          "fp8" if st.fp8 else "bf16", st.fp8_reason, "fp8" if st.fp8_dgrad else "bf16",
-                         st.fp8_dgrad_reason, "fp8" if st.fp8_wgrad else "bf16", st.fp8_wgrad_reason)
+                         st.fp8_dgrad_reason, "fp8" if st.fp8_wgrad else "bf16", st.fp8_wgrad_reason, tail)
         elif layer.type_name == "INNER_PRODUCT" and getattr(layer, "_sm100", None) is None:
             layer._sm100 = sm100.IPState(layer, tuple(net.blob_shapes[net.bottom_names[i][0]]))
 

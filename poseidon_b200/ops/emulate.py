@@ -68,6 +68,9 @@ def e5m2_quant(v: torch.Tensor, s) -> torch.Tensor:
     return torch.clamp(v.float() * s, -E5M2_MAX, E5M2_MAX).to(E5M2)
 
 
+AMAX_HISTORY = 16          # slots of a delayed-scaling amax ring (csrc/ops/fp8_quant.cu kAmaxHistory)
+
+
 def chwn_images(n: int) -> int:
     """Images per channel row of the fp8 weight gradient's batch-innermost copies: 16, 32, 64 or a multiple of 128."""
     if n <= 64:
@@ -329,6 +332,52 @@ class EmulatedKernels:
         """(e5m2 [C, OH, OW, Np], fp8_quant_grad's NHWC copy when nhwc else an empty tensor, the bf16 dY that was
         cast) (csrc/ops/fp8_quant.cu fp8_quant_grad_t)."""
         q, src = self.fp8_quant_grad(dy, s_out, y, slope)
+        return self._chwn(q), q if nhwc else torch.empty(0, dtype=E5M2), src
+
+    # ------------------------------------------------------------------------------------------ fp8 delayed scaling
+    @staticmethod
+    def _delayed_cast(v, s_out, ring, seed, scale_fn, quant_fn):
+        """One delayed-scaling call on the fp32 values v (csrc/ops/fp8_quant.cu, "Delayed scaling"): s from the amax of
+        the 15 history slots other than the position (seed: from v's own amax, then written into every slot), an infinite
+        element cast as NaN, v's amax recorded into the position's slot, the position advanced.  Returns the fp8 values."""
+        hist = ring[:AMAX_HISTORY].view(torch.float32)
+        pos = int(ring[AMAX_HISTORY])
+        amax = _nan_free_abs(v).amax() if v.numel() else torch.zeros(())
+        window = amax if seed else torch.cat([hist[:pos], hist[pos + 1:]]).amax()
+        s = scale_fn(window)
+        s_out.copy_(torch.div(torch.ones_like(s), s).reshape(s_out.shape))
+        q = quant_fn(torch.where(torch.isinf(v), torch.full_like(v, float("nan")), v), s)
+        if seed:
+            hist.fill_(float(amax))
+        else:
+            hist[pos] = amax
+        ring[AMAX_HISTORY] = (pos + 1) % AMAX_HISTORY
+        return q
+
+    def _delayed_nhwc(self, v, s_out, ring, seed, dtype, scale_fn, quant_fn):
+        n, c, h, w = v.shape
+        full = torch.zeros((n, (c + 15) // 16 * 16, h, w), dtype=dtype).contiguous(memory_format=CL)
+        full[:, :c].copy_(self._delayed_cast(v, s_out, ring, seed, scale_fn, quant_fn))
+        return full[:, :c]
+
+    def fp8_quant_act_delayed(self, x, s_out, ring, seed):
+        """fp8_quant_act with delayed scaling: ring int32 [AMAX_HISTORY + 3] (csrc/ops/fp8_quant.cu fp8_quant_act_delayed)."""
+        return self._delayed_nhwc(x.float(), s_out, ring, seed, E4M3, e4m3_scale, e4m3_quant)
+
+    def fp8_quant_act_t_delayed(self, x, s_out, ring, seed, nhwc):
+        """(the batch-innermost e4m3 copy, the NHWC copy when nhwc else an empty tensor), one scale for both
+        (csrc/ops/fp8_quant.cu fp8_quant_act_t_delayed)."""
+        q = self.fp8_quant_act_delayed(x, s_out, ring, seed)
+        return self._chwn(q), q if nhwc else torch.empty(0, dtype=E4M3)
+
+    def fp8_quant_grad_delayed(self, dy, s_out, ring, seed, y, slope):
+        """fp8_quant_grad with delayed scaling (csrc/ops/fp8_quant.cu fp8_quant_grad_delayed)."""
+        src = dy if y is None else _nhwc(torch.where(y.float() > 0, dy.float(), dy.float() * slope).to(BF16))
+        return self._delayed_nhwc(src.float(), s_out, ring, seed, E5M2, e5m2_scale, e5m2_quant), src
+
+    def fp8_quant_grad_t_delayed(self, dy, s_out, ring, seed, y, slope, nhwc):
+        """fp8_quant_grad_t with delayed scaling (csrc/ops/fp8_quant.cu fp8_quant_grad_t_delayed)."""
+        q, src = self.fp8_quant_grad_delayed(dy, s_out, ring, seed, y, slope)
         return self._chwn(q), q if nhwc else torch.empty(0, dtype=E5M2), src
 
     def conv_wgrad_fp8(self, dy8t, x8t, s_dy, s_x, dw, kernel, pad, groups, alpha, cgk):

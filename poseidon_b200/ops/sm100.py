@@ -137,6 +137,43 @@ def fp8_for_engine(engine: str, mode: Optional[str] = None) -> str:
     return "off"
 
 
+FP8_SCALINGS = ("current", "delayed")
+AMAX_HISTORY = 16                       # slots of a delayed-scaling amax ring (csrc/ops/fp8_quant.cu kAmaxHistory)
+_RING_WORDS = AMAX_HISTORY + 3          # + position, CTA ticket, running amax of the call in flight
+
+
+def resolve_fp8_scaling(scaling: Optional[str] = None, fp8: str = "off") -> str:
+    """How the fp8 quantisers of activations and dY choose their per-tensor scale: ``scaling`` when given, else
+    ``POSEIDON_FP8_SCALING`` when the fp8 mode ``fp8`` is on (unset, or fp8 "off": "current").
+    "current": just in time, from an amax pass over the tensor, then a cast pass.
+    "delayed": from the amax history of the tensor's previous quantiser calls in device memory, in one pass (DESIGN §17);
+    a tensor that grows past its history's amax saturates.  An explicit "delayed" with fp8 "off" is an error."""
+    if scaling is None:
+        if fp8 == "off":
+            return "current"
+        scaling = os.environ.get("POSEIDON_FP8_SCALING", "current")
+    m = str(scaling).lower()
+    if m not in FP8_SCALINGS:
+        raise ValueError(f"fp8_scaling must be one of {', '.join(FP8_SCALINGS)}, got '{m}'")
+    if m == "delayed" and fp8 == "off":
+        raise ValueError("fp8_scaling='delayed' needs an fp8 mode (fp8 is 'off')")
+    return m
+
+
+def fp8_scaling_for_engine(engine: str, fp8: str, scaling: Optional[str] = None) -> str:
+    """The fp8 scaling a net built for ``engine`` with the resolved fp8 mode ``fp8`` runs with.  Asking another engine for
+    delayed scaling explicitly is an error, and ``POSEIDON_FP8_SCALING`` does not apply to it."""
+    if engine == "sm100":
+        return resolve_fp8_scaling(scaling, fp8)
+    if scaling is not None:
+        m = str(scaling).lower()
+        if m not in FP8_SCALINGS:
+            raise ValueError(f"fp8_scaling must be one of {', '.join(FP8_SCALINGS)}, got '{m}'")
+        if m == "delayed":
+            raise ValueError(f"fp8_scaling='{scaling}' needs the sm100 engine (engine is '{engine}')")
+    return "current"
+
+
 def _round128(c: int) -> int:
     return (c + 127) // 128 * 128
 
@@ -147,7 +184,7 @@ def _round128(c: int) -> int:
 class ConvState:
     """Per-layer engine state: operand layouts + bf16 shadows, refreshed lazily by weight version."""
 
-    def __init__(self, layer, cin_logical: int, fp8: Optional[str] = None):
+    def __init__(self, layer, cin_logical: int, fp8: Optional[str] = None, fp8_scaling: Optional[str] = None):
         self.layer = layer
         self.groups = layer.group
         self.R, self.S = layer.kernel
@@ -224,6 +261,12 @@ class ConvState:
             self.fp8_wgrad, self.fp8_wgrad_reason = self._fp8_wgrad_eligible(layer)
         self.cgkw8 = _pad64(self.cg) if self.fp8_wgrad else 0
         self.s_xw: Optional[torch.Tensor] = None      # X's scale for the weight gradient (not the forward's s_x)
+        # delayed scaling (opt-in): the activation / dY quantisers of training passes scale from amax histories in device
+        # memory, one per scaled tensor ("x": the forward input, "dy", "xw": the weight gradient's X when the forward is
+        # bf16), each [int32 ring, seeded?]; never saved, so a resumed run seeds them again
+        self.fp8_delayed = resolve_fp8_scaling(fp8_scaling, mode) == "delayed" and \
+            (self.fp8 or self.fp8_dgrad or self.fp8_wgrad)
+        self.amax_rings: dict = {}
         self.wbp: Optional[torch.Tensor] = None      # channel-padded copy of wb (derived, refreshed when wb changes)
         self.dirty_wbp = True
         self.wb: Optional[torch.Tensor] = None
@@ -412,10 +455,10 @@ class ConvState:
         return dw.view(self.Cout, self.R, self.S, self.cg).permute(0, 3, 1, 2)   # channels-last strided view
 
 
-def conv_state(layer, cin_logical, fp8: Optional[str] = None) -> ConvState:
+def conv_state(layer, cin_logical, fp8: Optional[str] = None, fp8_scaling: Optional[str] = None) -> ConvState:
     st = getattr(layer, "_sm100", None)
     if st is None:
-        st = ConvState(layer, cin_logical, fp8)
+        st = ConvState(layer, cin_logical, fp8, fp8_scaling)
         layer._sm100 = st
     return st
 
@@ -458,7 +501,7 @@ def prepare_first_layer_input(x: torch.Tensor, st: ConvState, pad, in_hw) -> tor
 
 class _ConvFn(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, x, weight, bias, layer, relu_slope):
+    def forward(ctx, x, weight, bias, layer, relu_slope, delayed):
         st: ConvState = layer._sm100
         k = K()
         stride, pad = layer.stride, layer.pad
@@ -477,6 +520,7 @@ class _ConvFn(torch.autograd.Function):
         oh = (h + 2 * pad[0] - st.R) // stride[0] + 1
         ow = (w + 2 * pad[1] - st.S) // stride[1] + 1
         relu = relu_slope is not None
+        x8t = None                  # delayed scaling: the weight gradient's X copy, written by the forward's quantiser
         if st.s2d:
             y = k.conv_fprop(xin, st.shadow(), bias, [st.Rq, st.Sq], [1, 1], [0, 0], 1, 0, oh, ow, relu,
                              float(relu_slope or 0.0), None)
@@ -489,16 +533,16 @@ class _ConvFn(torch.autograd.Function):
             if slab is not None and st.Coutp == st.Cout:
                 out = slab[0].slab_view(slab[1], xin.shape[0], oh, ow, xin.device)
             if st.fp8:
-                y = _fp8_fprop(k, st, weight, xin, bias, list(stride), list(conv_pad), oh, ow, relu,
-                               float(relu_slope or 0.0), out)
+                y, x8t = _fp8_fprop(k, st, weight, xin, bias, list(stride), list(conv_pad), oh, ow, relu,
+                                    float(relu_slope or 0.0), out, delayed)
             else:
                 y = k.conv_fprop(xin, st.operand(), bias, [st.R, st.S], list(stride), list(conv_pad), st.groups,
                                  1 if (st.row_mode and not st.pad8) else 0, oh, ow, relu, float(relu_slope or 0.0), out)
             if st.Coutp != st.Cout:
                 y = y[:, : st.Cout]            # channel slice of the padded tensor (pixel pitch Coutp)
-        ctx.layer, ctx.relu_slope, ctx.conv_pad = layer, relu_slope, conv_pad
+        ctx.layer, ctx.relu_slope, ctx.conv_pad, ctx.delayed = layer, relu_slope, conv_pad, delayed
         ctx.in_shape = tuple(x.shape)
-        ctx.save_for_backward(xin, y if relu else None)
+        ctx.save_for_backward(xin, y if relu else None, x8t)
         return y
 
     @staticmethod
@@ -506,7 +550,7 @@ class _ConvFn(torch.autograd.Function):
         layer = ctx.layer
         st: ConvState = layer._sm100
         k = K()
-        xin, y = ctx.saved_tensors
+        xin, y, x8t = ctx.saved_tensors
         if st.Coutp != st.Cout:
             # zero-padded output channels: mask (if any) on the logical slice, then widen dY to the padded layout
             if y is not None and not st.consumer_masks:
@@ -521,11 +565,11 @@ class _ConvFn(torch.autograd.Function):
                 # e5m2 dY for the weight gradient (batch-innermost copy, plus the NHWC copy of an fp8 data gradient):
                 # one amax pass (ReLU backward fused in as below) and one cast pass, on this stream before the fork
                 dy8t, dy8, dy = _fp8_quant_grad_t(k, st, dy, y if not st.consumer_masks else None, ctx.relu_slope,
-                                                  st.fp8_dgrad and ctx.needs_input_grad[0])
+                                                  st.fp8_dgrad and ctx.needs_input_grad[0], ctx.delayed)
             elif st.fp8_dgrad and ctx.needs_input_grad[0]:
                 # e5m2 dY: amax pass (with this layer's ReLU backward fused in when it masks its own gradient; the
                 # weight / bias gradients below then read the masked bf16 dY it writes) and cast
-                dy8, dy = _fp8_quant_grad(k, st, dy, y if not st.consumer_masks else None, ctx.relu_slope)
+                dy8, dy = _fp8_quant_grad(k, st, dy, y if not st.consumer_masks else None, ctx.relu_slope, ctx.delayed)
             elif y is not None and not st.consumer_masks:
                 if y.is_contiguous(memory_format=CL) and dy.is_contiguous(memory_format=CL):
                     dy = k.relu_bwd(y, dy, float(ctx.relu_slope))
@@ -574,14 +618,23 @@ class _ConvFn(torch.autograd.Function):
             xin.record_stream(side)
             if st.fp8_wgrad and dw2 is not None:
                 dy8t.record_stream(side)
+                if x8t is not None:
+                    x8t.record_stream(side)
             torch.cuda.set_stream(side)
         try:
             if dw2 is not None:
                 if st.s2d:
                     k.conv_wgrad(xin, dy, dw2, [st.Rq, st.Sq], [1, 1], [0, 0], 1, 0, 1.0, 0)
+                elif st.fp8_wgrad and x8t is not None:
+                    # delayed scaling: the forward's quantiser wrote X's copy with the forward's scale
+                    k.conv_wgrad_fp8(dy8t, x8t, st.s_dy, st.s_x, dw2, [st.R, st.S], list(ctx.conv_pad), st.groups, 1.0,
+                                     st.cgkw8)
                 elif st.fp8_wgrad:
                     # e4m3 X (its own scale) and the fp8 GEMM, on the weight-gradient side stream
-                    x8t = k.fp8_quant_act_t(xin, st.s_xw)
+                    if ctx.delayed:
+                        x8t, _ = _delayed_quant(st, "xw", k.fp8_quant_act_t_delayed, xin, st.s_xw, False)
+                    else:
+                        x8t = k.fp8_quant_act_t(xin, st.s_xw)
                     k.conv_wgrad_fp8(dy8t, x8t, st.s_dy, st.s_xw, dw2, [st.R, st.S], list(ctx.conv_pad), st.groups, 1.0,
                                      st.cgkw8)
                 else:
@@ -625,33 +678,43 @@ class _ConvFn(torch.autograd.Function):
                 _pending_wgrad.setdefault(cur.device.index, []).append(done)
             else:
                 cur.wait_event(done)            # join: dw / db are complete for whoever consumes them on this stream
-        return dx, dw, db, None, None
+        return dx, dw, db, None, None, None
 
 
-def _fp8_fprop(k, st: ConvState, weight, xin, bias, stride, pad, oh, ow, relu, slope, out):
+def _fp8_fprop(k, st: ConvState, weight, xin, bias, stride, pad, oh, ow, relu, slope, out, delayed):
     """e4m3 forward: quantise the fp32 master and the input, then the fp8 im2col GEMM.  All three launches run on every
-    forward: under a CUDA graph Python does not run at replay, and the optimizer updates the master inside the graph."""
+    forward: under a CUDA graph Python does not run at replay, and the optimizer updates the master inside the graph.
+    Returns (y, the weight gradient's X copy written by the same pass under delayed scaling, else None)."""
     w = weight.detach()
     if st.s_x is None:
         st.s_x = torch.ones(1, device=w.device, dtype=torch.float32)
         st.s_w = torch.ones(st.Cout, device=w.device, dtype=torch.float32)
     w8 = k.fp8_quant_weight(w, st.cgk8, st.s_w)
-    x8 = k.fp8_quant_act(xin, st.s_x)
-    return k.conv_fprop_fp8(x8, w8, st.s_x, st.s_w, None if bias is None else bias.detach(), [st.R, st.S], stride, pad,
-                            st.groups, oh, ow, relu, slope, out)
+    x8t = None
+    if delayed and st.fp8_wgrad:
+        x8t, x8 = _delayed_quant(st, "x", k.fp8_quant_act_t_delayed, xin, st.s_x, True)
+    elif delayed:
+        x8 = _delayed_quant(st, "x", k.fp8_quant_act_delayed, xin, st.s_x)
+    else:
+        x8 = k.fp8_quant_act(xin, st.s_x)
+    y = k.conv_fprop_fp8(x8, w8, st.s_x, st.s_w, None if bias is None else bias.detach(), [st.R, st.S], stride, pad,
+                         st.groups, oh, ow, relu, slope, out)
+    return y, x8t
 
 
-def _fp8_quant_grad(k, st: ConvState, dy, y, slope):
+def _fp8_quant_grad(k, st: ConvState, dy, y, slope, delayed=False):
     """e5m2 dY for the fp8 data gradient: returns (dy8, the bf16 dY the weight / bias gradients read).  With y (the layer
     masks its own gradient) the amax pass applies the ReLU backward and writes the masked dY, bit-identical to relu_bwd.
     Runs on every backward (graph replays included); the scale tensors are allocated once per layer."""
     if st.s_dy is None:
         st.s_dy = torch.ones(1, device=dy.device, dtype=torch.float32)
         st.s_wt = torch.ones(st.Cp, device=dy.device, dtype=torch.float32)
+    if delayed:
+        return _delayed_quant(st, "dy", k.fp8_quant_grad_delayed, dy, st.s_dy, y, float(slope or 0.0))
     return k.fp8_quant_grad(dy, st.s_dy, y, float(slope or 0.0))
 
 
-def _fp8_quant_grad_t(k, st: ConvState, dy, y, slope, nhwc: bool):
+def _fp8_quant_grad_t(k, st: ConvState, dy, y, slope, nhwc: bool, delayed=False):
     """e5m2 dY for the fp8 weight gradient: returns (dy8t, dy8 for an fp8 data gradient (nhwc) else None, the bf16 dY the
     bias gradient reads), with the scale and mask of _fp8_quant_grad."""
     if st.s_dy is None:
@@ -659,8 +722,39 @@ def _fp8_quant_grad_t(k, st: ConvState, dy, y, slope, nhwc: bool):
         st.s_wt = torch.ones(st.Cp, device=dy.device, dtype=torch.float32)
     if st.s_xw is None:
         st.s_xw = torch.ones(1, device=dy.device, dtype=torch.float32)
-    dy8t, dy8, src = k.fp8_quant_grad_t(dy, st.s_dy, y, float(slope or 0.0), nhwc)
+    if delayed:
+        dy8t, dy8, src = _delayed_quant(st, "dy", k.fp8_quant_grad_t_delayed, dy, st.s_dy, y, float(slope or 0.0), nhwc)
+    else:
+        dy8t, dy8, src = k.fp8_quant_grad_t(dy, st.s_dy, y, float(slope or 0.0), nhwc)
     return dy8t, (dy8 if nhwc else None), src
+
+
+def _capturing() -> bool:
+    """Is the current CUDA stream being captured into a graph?"""
+    return torch.cuda.is_available() and torch.cuda.is_current_stream_capturing()
+
+
+def _delayed_quant(st: ConvState, key: str, op, x, s_out, *args):
+    """One delayed-scaling quantiser call op(x, s_out, ring, seed, *args) on the amax history ``key`` of this layer.  The
+    first call seeds the ring (amax pass, then every slot holds that amax: the just-in-time result).  Seeding happens on
+    eager steps: a CUDA graph would replay the seed on every step, so a capture that reaches an unseeded ring fails."""
+    entry = st.amax_rings.get(key)
+    if entry is None:
+        entry = st.amax_rings[key] = [torch.zeros(_RING_WORDS, dtype=torch.int32, device=x.device), False]
+    if not entry[1] and _capturing():
+        raise RuntimeError(f"sm100 conv '{st.layer.layer_name}': fp8_scaling='delayed' reached the unseeded amax history "
+                           f"'{key}' inside a CUDA-graph capture; run an eager training step first")
+    out = op(x, s_out, entry[0], not entry[1], *args)
+    entry[1] = True
+    return out
+
+
+def reset_amax_histories(net) -> None:
+    """Forget the delayed-scaling amax histories of ``net``'s convolutions (a restored run seeds them again)."""
+    for layer in net.layers:
+        st = getattr(layer, "_sm100", None)
+        if isinstance(st, ConvState):
+            st.amax_rings.clear()
 
 
 _DGRAD_PACK = os.environ.get("POSEIDON_DGRAD_PACK", "0") == "1"      # A/B switch: always use the packed dgrad operand
@@ -774,8 +868,11 @@ def _strided_dgrad(k, st: "ConvState", layer, dy: torch.Tensor, xin: torch.Tenso
 def conv2d(x, w, b, stride, pad, groups, relu_slope=None, layer=None):
     if layer is None or not _on(x):
         return TE.conv2d(x, w, b, stride, pad, groups, relu_slope, layer)
-    conv_state(layer, w.shape[1] * groups)
-    return _ConvFn.apply(x, w, b, layer, relu_slope)
+    st = conv_state(layer, w.shape[1] * groups)
+    # delayed scaling on training passes only: test-phase forwards (test nets share this layer's state) and forwards
+    # without autograd scale just in time and leave the amax histories alone
+    delayed = st.fp8_delayed and torch.is_grad_enabled() and layer.ctx.train
+    return _ConvFn.apply(x, w, b, layer, relu_slope, delayed)
 
 
 # =====================================================================================================

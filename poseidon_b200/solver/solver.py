@@ -93,7 +93,7 @@ class Solver:
                  comm: str = "auto", staleness: int = 0, svb: bool = False, grad_reduce: str = "sum",
                  dtype=None, model_dir: Optional[str] = None, data_shape_hint=None,
                  snapshot_dir: Optional[str] = None, sfb_mode: str = "auto", aggr_fraction: float = 0.1,
-                 wire_dtype: Optional[str] = None, fp8: Optional[str] = None):
+                 wire_dtype: Optional[str] = None, fp8: Optional[str] = None, fp8_scaling: Optional[str] = None):
         if isinstance(param, str):
             model_dir = model_dir or os.path.dirname(os.path.abspath(param))
             param = P.read_solver(param)
@@ -109,8 +109,9 @@ class Solver:
                 rank_ctx = RankContext()
         self.rank_ctx = rank_ctx
         self.engine = engine
-        from ..ops.sm100 import fp8_for_engine
+        from ..ops.sm100 import fp8_for_engine, fp8_scaling_for_engine
         self.fp8 = fp8_for_engine(engine, fp8)     # "fprop" / "fprop+dgrad" / "fprop+dgrad+wgrad" (ops/sm100.py)
+        self.fp8_scaling = fp8_scaling_for_engine(engine, self.fp8, fp8_scaling)      # "current" / "delayed"
         self.staleness = int(staleness)
         self.aggr_fraction = float(aggr_fraction)
         # gradients on the network as bf16 (the reference's DenseFloat16 row oplogs: fp16 on the wire, fp32 at rest);
@@ -153,7 +154,8 @@ class Solver:
         ctx = NetContext(phase=phase, device=dev, engine=self.engine, dtype=self.dtype,
                          rank=self.rank_ctx.rank, world_size=self.rank_ctx.world_size,
                          seed=None if seed is None else seed + self.rank_ctx.rank,
-                         data_shape_hint=self.data_shape_hint, model_dir=self.model_dir, fp8=self.fp8)
+                         data_shape_hint=self.data_shape_hint, model_dir=self.model_dir, fp8=self.fp8,
+                         fp8_scaling=self.fp8_scaling)
         return ctx
 
     def _resolve(self, path):
@@ -695,6 +697,9 @@ class Solver:
             raise ValueError("Incorrect length of history blobs.")
         for b, h, (layer, j) in zip(st.history, hs, self.net.param_owner):
             layer.import_blob(j, np.asarray(b.data, dtype=np.float32), tensor=h)
+        if self.fp8_scaling == "delayed":
+            from ..ops import sm100
+            sm100.reset_amax_histories(self.net)      # not in the snapshot: the resumed run seeds them on its first step
         if self.rank_ctx.is_root:
             log.info("Restored solver state from %s (iter %d)", fn, self.iter)
 

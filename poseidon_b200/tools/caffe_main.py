@@ -72,6 +72,10 @@ def make_parser():
                     help="sm100 engine: run eligible convolution forward passes on fp8 (e4m3) operands; fprop+dgrad: "
                          "also eligible stride-1 data gradients (e5m2 dY x e4m3 weights); fprop+dgrad+wgrad: also "
                          "eligible stride-1 weight gradients (e5m2 dY x e4m3 X) (default: POSEIDON_FP8, else off)")
+    ap.add_argument("--fp8_scaling", default=None, choices=["current", "delayed"],
+                    help="with an fp8 mode on: current scales activations and dY just in time (an amax pass, then a "
+                         "cast); delayed scales them from the amax history of their last 16 training steps in one pass, "
+                         "saturating values beyond it (default: POSEIDON_FP8_SCALING, else current)")
     ap.add_argument("--stats_json", default="")
     ap.add_argument("--log_level", default="INFO")
     for f in _PS_FLAGS:
@@ -148,7 +152,7 @@ def cmd_train(args) -> int:
                         model_dir=os.path.dirname(os.path.abspath(args.solver)), data_shape_hint=hint,
                         sfb_mode=args.sfb_mode, aggr_fraction=args.aggr_fraction,
                         wire_dtype=args.wire_dtype or ("bf16" if str(args.row_oplog_type) == "3" else None),
-                        fp8=args.fp8)
+                        fp8=args.fp8, fp8_scaling=args.fp8_scaling)
     if args.cuda_graph != "auto":
         solver.use_cuda_graph = args.cuda_graph == "1"
     if rc.is_root:
@@ -178,14 +182,16 @@ def _build_net(args, phase):
     from .. import proto as P
     from ..layers import NetContext
     from ..net.net import Net
-    from ..ops.sm100 import fp8_for_engine
+    from ..ops.sm100 import fp8_for_engine, fp8_scaling_for_engine
     dev = torch.device(f"cuda:{args.gpu.split(',')[0] or 0}" if (torch.cuda.is_available() and args.gpu != "-1") else "cpu")
     if dev.type == "cuda":
         torch.cuda.set_device(dev)
     engine = _engine(args, dev)
+    fp8 = fp8_for_engine(engine, args.fp8)
     ctx = NetContext(phase=phase, device=dev, engine=engine,
                      dtype=torch.bfloat16 if engine == "sm100" else torch.float32,
-                     model_dir=os.path.dirname(os.path.abspath(args.model)), fp8=fp8_for_engine(engine, args.fp8))
+                     model_dir=os.path.dirname(os.path.abspath(args.model)), fp8=fp8,
+                     fp8_scaling=fp8_scaling_for_engine(engine, fp8, args.fp8_scaling))
     if args.synthetic_shape:
         ctx.data_shape_hint = tuple(int(x) for x in args.synthetic_shape.lower().split("x"))
     net = Net(P.read_net(args.model), phase=phase, ctx=ctx)
