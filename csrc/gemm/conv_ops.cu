@@ -34,6 +34,8 @@ static int g_conv_im2col = 1;      // TMA im2col-mode operand fetch where the ge
 static int g_conv_cluster = 1;     // CTAs per cluster sharing the TMA operand by multicast (1 = off)
 
 int pair_cta_enabled();
+bool conv_dgrad_halo(const at::Tensor& dy, const at::Tensor& wb, int R, int S, int ph, int pw, int groups, int H, int W,
+                     const c10::optional<at::Tensor>& mask, double slope, at::Tensor& dx);
 extern int g_max_stages;
 extern int g_no_bulk_epi;
 
@@ -618,6 +620,9 @@ bool conv_dgrad_w_impl(const at::Tensor& dy, const at::Tensor& wb, at::IntArrayR
   const int Cout = wb.size(0), Cout_g = Cout / groups, RS = d.R * d.S;
   const int Cg = static_cast<int>(wb.size(1) / RS), Cin = Cg * groups;
   if (Cout_g % 8 != 0 || Cg % 8 != 0 || dv.C != Cout) return false;
+  // narrow input groups (AlexNet conv2): one dY halo per tile instead of one im2col tile per tap (halo_conv.cuh)
+  if (conv_dgrad_halo(dy, wb, d.R, d.S, d.ph, d.pw, d.groups, static_cast<int>(H), static_cast<int>(W), mask, slope, dx))
+    return true;
   const int Cok = (Cout_g + 63) / 64 * 64;
   NhwcView xv = nhwc_view(dx);
   auto stream = at::cuda::getCurrentCUDAStream();

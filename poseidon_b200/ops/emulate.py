@@ -113,6 +113,12 @@ class EmulatedKernels:
     def set_max_stages(self, n):
         return None
 
+    def set_conv_halo(self, mode):           # csrc/gemm/halo_conv.cu (schedule switch: bit-identical results)
+        return None
+
+    def conv_halo_launches(self):            # the emulated conv_dgrad_w has one schedule: never the halo kernel
+        return 0
+
     def set_pair_cta(self, on):              # csrc/gemm/gemm_ops.cu (cta_group::2 on/off: no numerical effect)
         return None
 

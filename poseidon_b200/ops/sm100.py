@@ -68,6 +68,8 @@ def K():
                 torch.ops.poseidon.set_conv_pair(int(env["POSEIDON_CONV_PAIR"]))
             if "POSEIDON_CONV_MCAST" in env:
                 torch.ops.poseidon.set_conv_mcast(int(env["POSEIDON_CONV_MCAST"]))
+            if "POSEIDON_CONV_HALO" in env:
+                torch.ops.poseidon.set_conv_halo(int(env["POSEIDON_CONV_HALO"]))
             if "POSEIDON_BULK_EPI" in env:
                 torch.ops.poseidon.set_bulk_epilogue(int(env["POSEIDON_BULK_EPI"]))
     return _ops
