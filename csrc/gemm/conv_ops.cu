@@ -36,6 +36,8 @@ static int g_conv_cluster = 1;     // CTAs per cluster sharing the TMA operand b
 int pair_cta_enabled();
 bool conv_dgrad_halo(const at::Tensor& dy, const at::Tensor& wb, int R, int S, int ph, int pw, int groups, int H, int W,
                      const c10::optional<at::Tensor>& mask, double slope, at::Tensor& dx);
+bool conv_fprop_halo(const at::Tensor& x, const at::Tensor& wb, const c10::optional<at::Tensor>& bias, int R, int S, int ph,
+                     int pw, int groups, bool relu, double slope, at::Tensor& y);
 extern int g_max_stages;
 extern int g_no_bulk_epi;
 
@@ -269,6 +271,21 @@ at::Tensor conv_fprop(const at::Tensor& x, const at::Tensor& wb, const c10::opti
   TORCH_CHECK(yv.C == Cout && yv.H == OH && yv.W == OW && yv.N == xv.N, "conv_fprop: bad output tensor");
   auto stream = at::cuda::getCurrentCUDAStream();
   const int sms = at::cuda::getCurrentDeviceProperties()->multiProcessorCount;
+  // narrow input groups (AlexNet conv2): one input halo per tile instead of one gathered A tile per k block (halo_conv.cuh),
+  // only where the gather kernel would run (stride-1 TAP mode, no channel-padded weights, no TMA im2col path)
+  if (d.mode == 0 && d.sh == 1 && d.sw == 1 && wb.size(1) == static_cast<int64_t>(d.R) * d.S * Cg) {
+    ConvGeom g0{};
+    g0.x = reinterpret_cast<const __nv_bfloat16*>(x.data_ptr());
+    g0.W = xv.W; g0.H = xv.H;
+    g0.pitch = xv.pitch;
+    g0.Cg = g0.Cgk = Cg;
+    g0.OH = static_cast<int>(OH); g0.OW = static_cast<int>(OW);
+    g0.R = d.R; g0.S = d.S;
+    g0.sh = g0.sw = 1;
+    g0.off_h = -d.ph; g0.off_w = -d.pw;
+    g0.dr = 1;
+    if (!im2col_ok(g0) && conv_fprop_halo(x, wb, bias, d.R, d.S, d.ph, d.pw, d.groups, relu, slope, y)) return y;
+  }
   for (int gidx = 0; gidx < groups; ++gidx) {
     // channel-padded operand (R*S*Cgk columns, Cgk = Cg rounded up to 64): the TMA im2col path zero-fills slots >= Cg
     const int Cgk = (d.mode == 0 && wb.size(1) != static_cast<int64_t>(d.R) * d.S * Cg) ? static_cast<int>(wb.size(1) / (d.R * d.S)) : 0;

@@ -1,4 +1,5 @@
-// Host side of the halo-tiled data gradient (halo_conv.cuh): geometry selection, tensor maps, launch, the A/B switch.
+// Host side of the halo-tiled data gradient and forward (halo_conv.cuh): geometry selection, tensor maps, launch, the A/B
+// switches.
 #include <ATen/cuda/CUDAContext.h>
 #include <c10/cuda/CUDAGuard.h>
 #include <torch/library.h>
@@ -169,6 +170,106 @@ bool conv_dgrad_halo(const at::Tensor& dy, const at::Tensor& wb, int R, int S, i
   return true;
 }
 
+// set_conv_halo_fprop: 0 off (gather schedule only), 1 where the geometry selects it (default), 2 wherever it can run
+static int g_conv_halo_fprop = 1;
+static std::atomic<int64_t> g_halo_fprop_launches{0};
+
+// Plan of the halo forward for one geometry; false when it does not apply.  The kernel runs stride-1 forwards with at most
+// 64 input channels per group in whole k16 steps per tap (Cg % 16 == 0), whole 64-channel blocks of output per group and
+// two halos that fit shared memory beside the B ring.  It is selected where it also has at least 3x3 taps, at most 30 %
+// padded tile rows and at least two CTA tiles per SM.
+static bool halo_fprop_plan(int N, int OH, int OW, int R, int S, int Cg, int Cout_g, int groups, int sms, HaloFpropParams* out,
+                            int* smem_out) {
+  if (!g_conv_halo_fprop || Cg % 16 != 0 || Cg > 64 || Cout_g % 64 != 0) return false;
+  const int P = OW + S - 1;
+  constexpr int M = 64 * (4 + 3);
+  int T = std::min(OH, M / P);
+  if (P > 256 || T < 1) return false;
+  const int tiles = (OH + T - 1) / T;
+  T = (OH + tiles - 1) / tiles;                 // same tile count, rows spread evenly
+  const int Hb = (M + (R - 1) * P + S - 1 + P - 1) / P;
+  const int HP = (Hb * P + 7) / 8 * 8;
+  const int slabs = Cg / 8;
+  const long smem = 1024L + kHaloStages * kHaloBStageBytes + 2L * slabs * HP * 16 + kHaloZeroBytes + kHaloBarBytes;
+  if (Hb > 256 || smem > kHaloSmemLimit) return false;
+  HaloFpropParams& p = *out;
+  p = HaloFpropParams{};
+  p.OH = OH; p.OW = OW;
+  p.P = P; p.T = T;
+  p.tiles_per_img = tiles;
+  p.num_tiles = N * tiles;
+  p.nblk = Cout_g / 64;
+  p.cblocks = groups * p.nblk;
+  p.S = S; p.Cg = Cg; p.Cout_g = Cout_g;
+  p.steps = R * S * Cg / 16;
+  p.kb_per_tile = (p.steps + 3) / 4;
+  p.slabs = slabs; p.Hb = Hb; p.HP = HP;
+  p.halo_bytes = static_cast<uint32_t>(slabs) * Hb * P * 16;
+  *smem_out = static_cast<int>(smem);
+  if (g_conv_halo_fprop == 2) return true;
+  return R * S >= 9 && static_cast<long>(tiles) * M * 10 <= 13L * OH * OW &&
+         static_cast<long>(p.num_tiles) * p.cblocks >= 2L * sms;
+}
+
+// conv_fprop on the halo schedule when the geometry selects it (see halo_fprop_plan); false (nothing launched) otherwise.
+// The caller has established a stride-1 TAP-mode convolution without channel-padded weights that the gather kernel would
+// run.  x: NHWC bf16 [N, groups * Cg, H, W]; wb: [groups * Cout_g][R][S][Cg]; y: NHWC bf16 [N, groups * Cout_g, OH, OW].
+bool conv_fprop_halo(const at::Tensor& x, const at::Tensor& wb, const c10::optional<at::Tensor>& bias, int R, int S, int ph,
+                     int pw, int groups, bool relu, double slope, at::Tensor& y) {
+  const NhwcView xv = nhwc_view(x), yv = nhwc_view(y);
+  const int Cg = xv.C / groups, Cout_g = yv.C / groups;
+  if ((xv.pitch * 2) % 16 != 0 || (reinterpret_cast<uintptr_t>(x.data_ptr()) & 15) != 0 || yv.pitch % 2 != 0 ||
+      (reinterpret_cast<uintptr_t>(y.data_ptr()) & 3) != 0 || (reinterpret_cast<uintptr_t>(wb.data_ptr()) & 15) != 0)
+    return false;
+  const int sms = at::cuda::getCurrentDeviceProperties()->multiProcessorCount;
+  HaloFpropParams p;
+  int smem = 0;
+  if (!halo_fprop_plan(xv.N, yv.H, yv.W, R, S, Cg, Cout_g, groups, sms, &p, &smem)) return false;
+  p.ph = ph;
+  p.pw = pw;
+  p.y = reinterpret_cast<__nv_bfloat16*>(y.data_ptr());
+  p.ldc = yv.pitch;
+  p.bias = bias.has_value() ? bias->data_ptr<float>() : nullptr;
+  p.relu = relu;
+  p.slope = static_cast<float>(slope);
+  const int K = R * S * Cg;
+  CUtensorMap hm, wm;
+  encode_halo_map(&hm, x.data_ptr(), xv, xv.C, p.P, p.Hb);
+  encode_tmap_2d(&wm, wb.data_ptr(), K, static_cast<int64_t>(groups) * Cout_g, K, 64, 32);
+  auto kern = halo_fprop_kernel<4, 3>;
+  static int resident = 0;
+  if (resident == 0) {
+    C10_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kHaloSmemLimit));
+    resident = resident_cluster_ctas(kern, kHaloThreads, kHaloSmemLimit, 2);
+  }
+  const long pair_tiles = static_cast<long>(p.num_tiles + 1) / 2 * p.cblocks;
+  const int grid = static_cast<int>(2 * std::max<long>(1, std::min<long>(pair_tiles, std::min(resident, sms) / 2)));
+  cudaLaunchConfig_t cfg{};
+  cfg.gridDim = dim3(grid);
+  cfg.blockDim = dim3(kHaloThreads);
+  cfg.dynamicSmemBytes = smem;
+  cfg.stream = at::cuda::getCurrentCUDAStream();
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeClusterDimension;
+  attr[0].val.clusterDim.x = 2;
+  attr[0].val.clusterDim.y = 1;
+  attr[0].val.clusterDim.z = 1;
+  cfg.attrs = attr;
+  cfg.numAttrs = 1;
+  C10_CUDA_CHECK(cudaLaunchKernelEx(&cfg, kern, hm, wm, p));
+  C10_CUDA_KERNEL_LAUNCH_CHECK();
+  g_halo_fprop_launches.fetch_add(1, std::memory_order_relaxed);
+  return true;
+}
+
+void set_conv_halo_fprop(int64_t mode) {
+  TORCH_CHECK(mode >= 0 && mode <= 2,
+              "set_conv_halo_fprop: 0 (off), 1 (where the geometry selects it) or 2 (wherever it can run)");
+  g_conv_halo_fprop = static_cast<int>(mode);
+}
+
+int64_t conv_halo_fprop_launches() { return g_halo_fprop_launches.load(std::memory_order_relaxed); }
+
 void set_conv_halo(int64_t mode) {
   TORCH_CHECK(mode >= 0 && mode <= 2, "set_conv_halo: 0 (off), 1 (where the geometry selects it) or 2 (wherever it can run)");
   g_conv_halo = static_cast<int>(mode);
@@ -181,4 +282,6 @@ int64_t conv_halo_launches() { return g_halo_launches.load(std::memory_order_rel
 TORCH_LIBRARY_FRAGMENT(poseidon, m) {
   m.def("set_conv_halo(int mode) -> ()", &psd::set_conv_halo);
   m.def("conv_halo_launches() -> int", &psd::conv_halo_launches);
+  m.def("set_conv_halo_fprop(int mode) -> ()", &psd::set_conv_halo_fprop);
+  m.def("conv_halo_fprop_launches() -> int", &psd::conv_halo_fprop_launches);
 }

@@ -119,6 +119,12 @@ class EmulatedKernels:
     def conv_halo_launches(self):            # the emulated conv_dgrad_w has one schedule: never the halo kernel
         return 0
 
+    def set_conv_halo_fprop(self, mode):     # csrc/gemm/halo_conv.cu (schedule switch: bit-identical results)
+        return None
+
+    def conv_halo_fprop_launches(self):      # the emulated conv_fprop has one schedule: never the halo kernel
+        return 0
+
     def set_pair_cta(self, on):              # csrc/gemm/gemm_ops.cu (cta_group::2 on/off: no numerical effect)
         return None
 

@@ -70,6 +70,8 @@ def K():
                 torch.ops.poseidon.set_conv_mcast(int(env["POSEIDON_CONV_MCAST"]))
             if "POSEIDON_CONV_HALO" in env:
                 torch.ops.poseidon.set_conv_halo(int(env["POSEIDON_CONV_HALO"]))
+            if "POSEIDON_CONV_HALO_FPROP" in env:
+                torch.ops.poseidon.set_conv_halo_fprop(int(env["POSEIDON_CONV_HALO_FPROP"]))
             if "POSEIDON_BULK_EPI" in env:
                 torch.ops.poseidon.set_bulk_epilogue(int(env["POSEIDON_BULK_EPI"]))
     return _ops
