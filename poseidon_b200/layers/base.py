@@ -71,6 +71,7 @@ class Layer(nn.Module):
     max_tops: Optional[int] = None
     is_loss = False
     is_data = False
+    label_tops: Sequence[int] = ()     # data layers: tops that carry labels (never made differentiable by force_backward)
 
     def __init__(self, lp, ctx: NetContext):
         super().__init__()
@@ -96,6 +97,11 @@ class Layer(nn.Module):
             raise ValueError(f"{self.type_name} layer '{n}' produces at least {self.min_tops} top blob(s)")
         if self.max_tops is not None and n_top > self.max_tops:
             raise ValueError(f"{self.type_name} layer '{n}' produces at most {self.max_tops} top blob(s)")
+
+    def allow_force_backward(self, bottom: int) -> bool:
+        """May a net's force_backward ask this layer for the diff of bottom ``bottom``?
+        reference: include/caffe/layer.hpp:296-298 (and the loss layers' overrides)."""
+        return True
 
     def add_blob(self, attr: str, shape: Shape, filler=None) -> nn.Parameter:
         t = torch.empty(shape, dtype=torch.float32)

@@ -64,6 +64,7 @@ class BasePrefetchingDataLayer(Layer):
     min_tops = 1
     max_tops = 2
     is_data = True
+    label_tops = (1,)
 
     def make_source(self):
         raise NotImplementedError
@@ -221,6 +222,7 @@ class HDF5DataLayer(Layer):
     exact_bottoms = 0
     exact_tops = 2
     is_data = True
+    label_tops = (1,)
 
     def _load(self, path):
         if path.endswith(".npz") or path.endswith(".npy"):
@@ -306,6 +308,7 @@ class MemoryDataLayer(Layer):
     exact_bottoms = 0
     exact_tops = 2
     is_data = True
+    label_tops = (1,)
 
     def setup(self, bottom_shapes):
         mp = self.lp.memory_data_param

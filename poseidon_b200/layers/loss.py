@@ -29,6 +29,10 @@ class LossLayer(Layer):
     def configure(self, bottom_shapes):
         pass
 
+    def allow_force_backward(self, bottom: int) -> bool:
+        """The label (bottom 1) is never forced.  reference: include/caffe/loss_layers.hpp:123-125."""
+        return bottom != 1
+
 
 @register("SOFTMAX_LOSS")
 class SoftmaxWithLossLayer(LossLayer):
@@ -54,6 +58,10 @@ class SoftmaxWithLossLayer(LossLayer):
 @register("EUCLIDEAN_LOSS")
 class EuclideanLossLayer(LossLayer):
     """reference: src/caffe/layers/euclidean_loss_layer.cpp:30-46."""
+
+    def allow_force_backward(self, bottom: int) -> bool:
+        """Both bottoms may be computed blobs.  reference: include/caffe/loss_layers.hpp:259-261."""
+        return True
 
     def forward(self, a, b):
         return (ops.reference.euclidean_loss(a, b.reshape(a.shape)),)
@@ -116,6 +124,10 @@ class ContrastiveLossLayer(LossLayer):
 
     def configure(self, bottom_shapes):
         self.margin = float(self.lp.contrastive_loss_param.margin)
+
+    def allow_force_backward(self, bottom: int) -> bool:
+        """The similarity label (bottom 2) is never forced.  reference: include/caffe/loss_layers.hpp:170-172."""
+        return bottom != 2
 
     def forward(self, a, b, sim):
         return (ops.reference.contrastive_loss(a, b, sim, self.margin),)

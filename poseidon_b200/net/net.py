@@ -203,6 +203,8 @@ class Net(nn.Module):
         self.layer_by_name = {n: l for n, l in zip(self.layer_names, self.layers)}
         self.blobs: Dict[str, torch.Tensor] = {}
         self.force_backward = bool(pd.force_backward)
+        self._plan_backward()
+        self._loss = None
         self.debug_info = False
         self.skip_layer = [False] * len(self.layers)
         if self.ctx.engine == "sm100":
@@ -212,6 +214,43 @@ class Net(nn.Module):
                 plan_sm100(self)
         from .lanes import default_lanes, plan_lanes
         plan_lanes(self, default_lanes(self.ctx))
+
+    def _plan_backward(self):
+        """``blob_need_backward``: which blobs get a diff, by the reference's rules (src/caffe/net.cpp:80-220).  A layer
+        needs backward when it has a parameter with a non-zero learning rate (every parameter counts when blobs_lr is
+        not given) or a bottom that needs backward; then all its tops do.  force_backward then marks every bottom a
+        layer allows (Layer.allow_force_backward: not a loss layer's label).  Net inputs and data-layer tops that end up
+        needing backward, labels excepted, become autograd leaves in forward() (only with force_backward)."""
+        need: Dict[str, bool] = {n: False for n in self.input_names}
+        for li, (lp, layer) in enumerate(zip(self.param_def.layers, self.layers)):
+            bnames = self.bottom_names[li]
+            lrs = [float(x) for x in lp.blobs_lr]
+            layer_needs = any(need[b] for b in bnames) or (any(lr > 0 for lr in lrs) if lrs else bool(layer.blob_names))
+            for t in self.top_names[li]:
+                need[t] = layer_needs or (t in bnames and need[t])      # an in-place top keeps its own flag
+        if self.force_backward:
+            for li, layer in enumerate(self.layers):
+                for j, b in enumerate(self.bottom_names[li]):
+                    if layer.allow_force_backward(j):
+                        need[b] = True
+        self.blob_need_backward: Dict[str, bool] = need
+        leaves = []
+        if self.force_backward:
+            leaves = [n for n in self.input_names if need[n]]
+            for li, layer in enumerate(self.layers):
+                if getattr(layer, "is_data", False):
+                    leaves += [t for j, t in enumerate(self.top_names[li]) if need[t] and j not in layer.label_tops]
+        self._grad_leaves = set(leaves)
+
+    @staticmethod
+    def _leaf(t: torch.Tensor) -> torch.Tensor:
+        return t.detach().requires_grad_(True) if t.is_floating_point() else t
+
+    def _data_outs(self, i: int, outs):
+        """A data layer's tops, the ones force_backward wants a diff of as autograd leaves."""
+        if not self._grad_leaves or not getattr(self.layers[i], "is_data", False):
+            return outs
+        return tuple(self._leaf(o) if t in self._grad_leaves else o for t, o in zip(self.top_names[i], outs))
 
     def _consumed_later(self, blob: str) -> bool:
         last_prod = max(i for i, tn in enumerate(self.top_names) if blob in tn)
@@ -231,6 +270,9 @@ class Net(nn.Module):
         for n in self.input_names:
             if n not in blobs:
                 raise ValueError(f"missing net input '{n}'")
+        for n in self._grad_leaves:           # (force_backward) every pass starts from fresh leaves
+            if n in blobs:
+                blobs[n] = self._leaf(blobs[n])
         end = len(self.layers) - 1 if end is None else end
         loss = None
         lanes = self._lane_runner(start, end)
@@ -242,7 +284,7 @@ class Net(nn.Module):
                 continue                      # fused into the producer's epilogue (in-place layer: blob unchanged)
             layer = self.layers[i]
             ins = [blobs[b] for b in self.bottom_names[i]]
-            outs = layer(*ins)
+            outs = self._data_outs(i, layer(*ins))
             for t, o, w in zip(self.top_names[i], outs, self.loss_weights[i]):
                 blobs[t] = o
                 if w != 0.0:
@@ -251,6 +293,7 @@ class Net(nn.Module):
             if self.debug_info:
                 self._forward_debug(i, outs)
         self.blobs = blobs if keep_blobs else {}
+        self._loss = loss if keep_blobs else None
         outputs = {n: blobs[n] for n in self.output_names if n in blobs}
         return loss, outputs
 
@@ -268,7 +311,7 @@ class Net(nn.Module):
                     torch.cuda.set_stream(lanes.streams[lane])
                     cur_lane = lane
                 lanes.before(i)
-                outs = self.layers[i](*[blobs[b] for b in self.bottom_names[i]])
+                outs = self._data_outs(i, self.layers[i](*[blobs[b] for b in self.bottom_names[i]]))
                 for t, o, w in zip(self.top_names[i], outs, self.loss_weights[i]):
                     blobs[t] = o
                     if w != 0.0:
@@ -322,6 +365,58 @@ class Net(nn.Module):
                 from ..ops import sm100
                 sm100.wait_pending_wgrad(clear=True)     # weight gradients forked to side streams join here
         return loss, outputs
+
+    def backward(self, top_diffs: Optional[Dict[str, torch.Tensor]] = None) -> Dict[str, torch.Tensor]:
+        """Backpropagate through the last forward pass: from ``top_diffs`` (blob name -> diff of that blob) when given,
+        else from the loss.  Parameter gradients accumulate into ``p.grad`` as in forward_backward().  Returns the diff
+        of every net input and data-layer top that needs backward (``blob_need_backward``; with force_backward off,
+        none), as float32 in the blob's logical NCHW shape whatever layout the engine ran it in.
+        reference: src/caffe/net.cpp:752-784 (Backward), python/caffe/pycaffe.py (net.backward(**diffs))."""
+        if not self.blobs:
+            raise RuntimeError("Net.backward() needs a forward pass that kept its blobs")
+        roots, seeds = [], []
+        for name, g in (top_diffs or {}).items():
+            t = self.blobs.get(name)
+            if t is None:
+                raise ValueError(f"'{name}' is not a blob of the last forward pass")
+            g = torch.as_tensor(g)
+            shapes = (tuple(t.shape), tuple(self.blob_shapes.get(name, t.shape)))
+            if tuple(g.shape) not in shapes or g.numel() != t.numel():
+                raise ValueError(f"diff for '{name}' has shape {tuple(g.shape)}; the blob has shape {shapes[1]}")
+            if t.requires_grad:
+                roots.append(t)
+                seeds.append(g.detach().to(device=t.device, dtype=t.dtype).reshape(t.shape))
+        if not top_diffs and self._loss is not None and self._loss.requires_grad:
+            roots.append(self._loss)
+            seeds.append(torch.ones_like(self._loss))
+        leaves = {n: self.blobs[n] for n in sorted(self._grad_leaves) if n in self.blobs and self.blobs[n].requires_grad}
+        for t in leaves.values():
+            t.grad = None
+        if roots:
+            torch.autograd.backward(roots, seeds)
+            if self.ctx.engine == "sm100":
+                from ..ops import sm100
+                sm100.wait_pending_wgrad(clear=True)     # weight gradients forked to side streams join here
+        return {n: self._logical_diff(n, t) for n, t in leaves.items()}
+
+    def _logical_diff(self, name: str, leaf: torch.Tensor) -> torch.Tensor:
+        """The diff of a net input / data-layer top as float32 in the blob's logical shape.  On the sm100 engine a data
+        layer may have handed its first convolution the physical s2d / ROW / 8-channel layout: first_layer_diff maps
+        that convolution's data gradient back."""
+        g = leaf.grad
+        logical = tuple(self.blob_shapes[name]) if name not in self.input_names else tuple(leaf.shape)
+        if g is None:
+            return torch.zeros(logical, dtype=torch.float32, device=leaf.device)
+        if tuple(g.shape) == logical:
+            return g.detach().float()
+        conv = None
+        for i, layer in enumerate(self.layers):
+            if getattr(layer, "is_data", False) and self.top_names[i][:1] == [name]:
+                conv = getattr(layer, "first_conv", None)
+        if conv is None:
+            raise RuntimeError(f"blob '{name}': diff of shape {tuple(g.shape)} for a blob of shape {logical}")
+        from ..ops import sm100
+        return sm100.first_layer_diff(g.detach(), conv, logical, True)
 
     def zero_grad_(self):
         for p in self.params:

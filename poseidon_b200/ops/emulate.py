@@ -477,6 +477,24 @@ class EmulatedKernels:
             return t.to(BF16).permute(0, 3, 1, 2)
         return _nhwc(t.to(BF16))
 
+    def first_layer_diff(self, src, C, H, W, ph, pw, s2d, out_float):
+        """A first-layer data gradient in the layout transform_nhwc wrote for that layer -> logical [N, C, H, W]
+        contiguous, fp32 or bf16 (csrc/ops/first_layer_diff.cu): the crop of the padded channels / spatial pre-padding, or
+        dx[n, c, y, x] = src[n, ((y+p)%4)*16 + ((x+p)%4)*4 + c, (y+p)/4, (x+p)/4] for space-to-depth.  A pure gather."""
+        assert src.dtype == BF16
+        n = src.shape[0]
+        if s2d:
+            assert src.shape[1] == 64 and C <= 4 and ph == pw
+            hq, wq = src.shape[2], src.shape[3]
+            t = src.permute(0, 2, 3, 1).reshape(n, hq, wq, 4, 4, 4)           # n, Y, X, dy, dx, c
+            t = t.permute(0, 5, 1, 3, 2, 4).reshape(n, 4, 4 * hq, 4 * wq)       # n, c, 4Y+dy, 4X+dx
+            t = t[:, :C]
+        else:
+            t = src[:, :C]
+        out = t[:, :, ph: ph + H, pw: pw + W]
+        assert tuple(out.shape[2:]) == (H, W), "first_layer_diff: source smaller than the logical blob"
+        return out.to(torch.float32 if out_float else BF16).contiguous()
+
     # ------------------------------------------------------------------------------------------ LRN / pooling
     def lrn_fwd(self, x, size, alpha, beta, fuse_relu):
         xf = x.float()

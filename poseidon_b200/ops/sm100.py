@@ -545,7 +545,7 @@ class _ConvFn(torch.autograd.Function):
             if st.Coutp != st.Cout:
                 y = y[:, : st.Cout]            # channel slice of the padded tensor (pixel pitch Coutp)
         ctx.layer, ctx.relu_slope, ctx.conv_pad, ctx.delayed = layer, relu_slope, conv_pad, delayed
-        ctx.in_shape = tuple(x.shape)
+        ctx.in_shape, ctx.in_dtype = tuple(x.shape), x.dtype
         ctx.save_for_backward(xin, y if relu else None, x8t)
         return y
 
@@ -655,10 +655,13 @@ class _ConvFn(torch.autograd.Function):
         if dbf is not None and defer and not defer_bias:
             db = bias_grad()                    # (multi-GPU: staged into the arena on this stream by the bucket launch)
         if ctx.needs_input_grad[0]:
-            if st.row_mode and not st.pad8:
-                raise NotImplementedError(f"sm100 conv '{layer.layer_name}': ROW-mode (<= 4 channel) layers are image "
-                                          "layers; their data gradient is never needed")
-            if tuple(stride) != (1, 1):
+            # dX comes back in the layout of the tensor the forward received: the physical s2d / ROW / 8-channel input a
+            # data layer handed over as it is, a logical input (deploy `input:`, LeNet conv2) through first_layer_diff
+            if st.s2d:
+                dx = _s2d_dgrad(k, st, layer, dy)
+            elif st.row_mode and not st.pad8:
+                dx = _strided_dgrad(k, st, layer, dy, xin, row=True)[:, : st.Cp]
+            elif tuple(stride) != (1, 1):
                 dx = _strided_dgrad(k, st, layer, dy, xin)
             else:
                 mask = xin if st.mask_input else None
@@ -675,8 +678,8 @@ class _ConvFn(torch.autograd.Function):
                 else:
                     dx = k.conv_dgrad(dy, st.dgrad_pack(), [st.R, st.S], list(layer.pad), st.groups, xin.shape[2],
                                       xin.shape[3], mask, 0.0)
-            if st.pad8 and st.Cp != st.cin_logical:
-                dx = dx[:, : st.cin_logical]
+            if tuple(dx.shape) != ctx.in_shape:
+                dx = first_layer_diff(dx, layer, ctx.in_shape, ctx.in_dtype == torch.float32)
         if done is not None:
             if defer:
                 _pending_wgrad.setdefault(cur.device.index, []).append(done)
@@ -811,20 +814,51 @@ def _wgrad_stream(cur: "torch.cuda.Stream") -> "torch.cuda.Stream":
 
 def _dgrad_reads_fprop_weights(st: "ConvState", layer, dy: torch.Tensor) -> bool:
     """Geometry the pack-free dgrad kernel covers (csrc/gemm/conv_ops.cu conv_dgrad_w): TAP-mode weights, channel counts
-    per group that are multiples of 8 (16-byte TMA strides), im2col-descriptor offsets within a signed byte."""
-    if _DGRAD_PACK or st.row_mode or st.pad8 or st.s2d or st.Coutp != st.Cout:
+    per group that are multiples of 8 (16-byte TMA strides), im2col-descriptor offsets within a signed byte.  An s2d layer
+    is asked about its 3x3 / pad-0 problem over 64 channels."""
+    if _DGRAD_PACK or (st.row_mode and not st.s2d) or st.pad8 or st.Coutp != st.Cout:
         return False
-    if st.cg % 8 != 0 or (st.Cout // st.groups) % 8 != 0:
+    if st.s2d:
+        cg, kernel, pad = 64, (st.Rq, st.Sq), (0, 0)
+    else:
+        cg, kernel, pad = st.cg, (st.R, st.S), layer.pad
+    if cg % 8 != 0 or (st.Cout // st.groups) % 8 != 0:
         return False
-    if max(st.R, st.S, layer.pad[0], layer.pad[1]) > 64:
+    if max(kernel[0], kernel[1], pad[0], pad[1]) > 64:
         return False
     pitch = dy.stride(3) if dy.shape[3] > 1 else (dy.stride(2) if dy.shape[2] > 1 else dy.stride(0))
     return dy.stride(1) == 1 and pitch % 8 == 0 and dy.data_ptr() % 16 == 0
 
 
-def _strided_dgrad(k, st: "ConvState", layer, dy: torch.Tensor, xin: torch.Tensor) -> torch.Tensor:
+def _s2d_dgrad(k, st: "ConvState", layer, dy: torch.Tensor) -> torch.Tensor:
+    """Data gradient of a space-to-depth first layer: the stride-1 data gradient of its 3x3 / pad-0 convolution over the
+    64 s2d channels, [N, 64, hq, wq] like the s2d input.  The shadow is zero at taps outside the 11x11 support and at the
+    padded 4th channel, so the padding lanes receive exact zeros."""
+    hq, wq = st.s2d_hw
+    dy = as_kernel_input(dy)
+    if _dgrad_reads_fprop_weights(st, layer, dy):
+        return k.conv_dgrad_w(dy, st.shadow(), [st.Rq, st.Sq], [0, 0], 1, hq, wq, None, 0.0)
+    if st.wt is None or st.dirty_wt:
+        st.wt = k.conv_pack_dgrad(st.shadow().float().reshape(-1), st.Cout, st.Rq * st.Sq, 64, 1, st.wt, 0)
+        st.dirty_wt = False
+    return k.conv_dgrad(dy, st.wt, [st.Rq, st.Sq], [0, 0], 1, hq, wq, None, 0.0)
+
+
+def first_layer_diff(dx: torch.Tensor, layer, shape, out_float: bool = True) -> torch.Tensor:
+    """A convolution's data gradient in its physical input layout (s2d, spatially pre-padded ROW, padded channels) ->
+    the logical blob's [N, C, H, W], contiguous, fp32 (``out_float``) or bf16.  Exact: a gather."""
+    st: ConvState = layer._sm100
+    n, c, h, w = shape
+    ph, pw = layer.pad if (st.s2d or (st.row_mode and not st.pad8)) else (0, 0)
+    return K().first_layer_diff(as_kernel_input(dx), c, h, w, ph, pw, st.s2d, out_float)
+
+
+def _strided_dgrad(k, st: "ConvState", layer, dy: torch.Tensor, xin: torch.Tensor, row: bool = False) -> torch.Tensor:
     """Data gradient of a strided convolution as sh * sw stride-1 problems (reference: any stride through col2im,
     src/caffe/layers/conv_layer.cu:84-119 + util/im2col.cu:74-113).
+    ``row``: a ROW-mode first layer, whose input is spatially pre-padded with 4 channels and which runs with pad 0: the
+    problem is posed over the pre-padded extent with pad 0 and the weight zero-padded to 8 input channels (the kernels'
+    channel granule); the result is an 8-channel dX over the padded extent.
 
     Input row ih = a + sh * i' (phase a) only receives taps r = r0 + sh * j with r0 = (a + ph) mod sh, and then
         oh = (ih + ph - r) / sh = i' + q - j,          q = (a + ph - r0) / sh   (an integer >= 0),
@@ -832,13 +866,13 @@ def _strided_dgrad(k, st: "ConvState", layer, dy: torch.Tensor, xin: torch.Tenso
     padding (q_h, q_w): the same wgmma dgrad kernel, one launch per phase, each writing one interleaved sub-grid of dX.
     No atomics, no col2im scatter."""
     sh, sw = layer.stride
-    ph, pw = layer.pad
+    ph, pw = (0, 0) if row else layer.pad
     n, _, H, W = xin.shape
-    cin = st.Cp
+    cin = 8 if row else st.Cp
     dx = torch.empty((n, cin, H, W), device=dy.device, dtype=torch.bfloat16, memory_format=CL)
     w4 = layer.weight.data.permute(0, 2, 3, 1)                       # [Cout, R, S, Cg] (physical order of the master)
-    if st.pad8:
-        w4 = torch.nn.functional.pad(w4, (0, st.Cp - st.cin_logical))
+    if st.pad8 or row:
+        w4 = torch.nn.functional.pad(w4, (0, cin - st.cin_logical))
     cg = w4.shape[3]
     packs = getattr(st, "_phase_packs", None)
     if packs is None or st.dirty_wt:
